@@ -1,12 +1,18 @@
 #!/usr/bin/env python
 """bench.py -- headline metric of BASELINE.json: SGEMM TFLOP/s (2*M*N*K / t) at M=N=K=8192.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   (N > 1: launched by torch.distributed.run, one rank per GPU)
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step computed -- a fixed, seeded sample of
+1024 rows of C (float32, 32 MB), c_rows.npy, and the indices of those rows, c_row_index.npy (float64) -- so that two builds
+can be compared output for output (the inputs are generated on the device from fixed seeds).  At N > 1 the rows are
+those of rank 0's panel of C (rows 0 .. 8191 of the global product); the other ranks write nothing.  The reference arm
+(--impl reference) refuses the flag: it times a CPU sample, not the GPU step.
 
 A "step" is one pass of the hot path: C <- A x B, fp32, row-major, alpha=1, beta=0 (the call the reference's bench
 makes, benchmarks/gemm/gemm_bench_float32.nim:184-189), through the C ABI of liblaser_b200.so in its DEFAULT fp32 mode
-(F16X3: tcgen05 kind::f16 over two fp16 pieces of the scaled operands, three passes, parity-gated at 1e-4).  At N GPUs
+(F16X3: wgmma f16 over two fp16 pieces of the scaled operands, three passes, parity-gated at 1e-4).  At N GPUs
 the headline line is weak-scaling: every rank owns 8192 rows of A and C, and each step includes B travelling over NCCL from
 rank 0 (prepared there, sent in column panels), issued by the library itself (laser_b200_gemm_rowsharded_f32_dev).
 
@@ -37,30 +43,21 @@ MNK = 8192
 STRONG_M = 32768
 
 
-def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the default kernel at 8192^3, from the committed
-    single-pass ncu capture (profiles/r02_traffic.json names the capture file it was read from); None if absent."""
-    path = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if not os.path.exists(path):
-        return None, None
-    t = json.load(open(path))
-    return float(t["dram_bytes_read"]) + float(t["dram_bytes_write"]), t.get("source")
-
-
 def load_peaks():
-    """MEASURED_PEAKS.json (driver-written).  The fp32 path runs on the tensor pipe whose TF32 rate is half the bf16 /
-    fp16 rate (UMMA K = 8 vs 16 per instruction at the same issue rate), so the fp32 tensor-core peak is taken as
-    measured bf16 / 2."""
+    """MEASURED_PEAKS.json when present.  The fp32 path runs on the tensor pipe whose TF32 rate is half the bf16 /
+    fp16 rate (wgmma K = 8 vs 16 per instruction at the same issue rate), so the fp32 tensor-core peak is taken as
+    bf16 / 2."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(bf16=float(p["bf16_tflops"]), bf16_sustained=float(p.get("bf16_tflops_sustained", p["bf16_tflops"])),
                     hbm=float(p["hbm_gbs"]), source="measured")
-    return dict(bf16=1590.0, bf16_sustained=1400.0, hbm=6650.0, source="fallback")  # B200_PROFILING.md
+    # fallback: NVIDIA's H100 SXM data sheet (dense bf16, HBM3), for a card allowed 700 W -- an upper bound, not a measured rate
+    return dict(bf16=989.0, bf16_sustained=989.0, hbm=3350.0, source="fallback")
 
 
 class ClockSampler:
-    """nvidia-smi samples during the timed region (recipe of B200_PROFILING.md)."""
+    """nvidia-smi samples during the timed region (clock, power, throttle reasons)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -344,6 +341,8 @@ def run_ours(args):
     n0 = L.launch_count()
     ms_step = timed(step, args.steps, 0)
     launches = L.launch_count() - n0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, C.view(M, N))
     # kernel-level roofline numbers: the same step, bracketed by CUDA events inside the library (profile mode disables the
     # dependent launch of the GEMM kernel, so it is measured separately from the headline time above)
     L.profile_begin()
@@ -374,20 +373,17 @@ def run_ours(args):
         flops_launch = 2.0 * M * N * K / max(1, prof["gemm_launches"] // prof_steps)   # algorithmic flops of one launch
         achieved = flops_launch / (gemm_ms * 1e-3) / 1e12
         tf32_peak = peaks["bf16"] / 2.0
-        traffic, traffic_src = load_traffic()
-        roofline = {"bound": "tensor", "kernel": "gemm_tc_kernel<fp16 pieces, 3 passes, CTA pair, scaled epilogue> (F16X3)",
+        roofline = {"bound": "tensor", "kernel": "gemm_tc_kernel<fp16 pieces, 3 passes, scaled epilogue> (F16X3)",
                     "achieved": achieved, "peak": tf32_peak, "unit": "TFLOP/s", "frac": achieved / tf32_peak,
-                    "traffic": traffic, "traffic_source": traffic_src,
-                    "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst) / 2 = fp32 (TF32-rate) tensor peak, of %s" % peaks["source"],
+                    "peak_source": ("MEASURED_PEAKS.json bf16_tflops (burst) / 2 = fp32 (TF32-rate) tensor peak" if peaks["source"] == "measured"
+                                    else "no MEASURED_PEAKS.json: H100 SXM data-sheet dense bf16 989 TFLOP/s (700 W) / 2 = TF32 495 TFLOP/s"),
                     "tensor_pipe_frac": 1.5 * achieved / tf32_peak,
                     "frac_of_sustained_peak": achieved / (peaks["bf16_sustained"] / 2.0),
                     "sustained_note": "kernel_ms is the CUDA-event time of the kernel inside a long back-to-back sequence (the part is at its power "
-                                      "cap by then); B200_PROFILING.md pairs such a time with the SUSTAINED cuBLAS figure (bf16_tflops_sustained / 2): "
-                                      "frac_of_sustained_peak.  `frac` keeps the stricter burst denominator used in round 1",
+                                      "cap by then); frac_of_sustained_peak divides by bf16_tflops_sustained / 2 of MEASURED_PEAKS.json when present",
                     "note": "achieved counts ALGORITHMIC flops 2MNK; the default mode issues three fp16 MMAs (K = 16 each, the bf16 "
                             "rate) per useful MAC = 1.5 TF32-equivalents, so frac <= 2/3 by construction and tensor_pipe_frac = "
-                            "1.5 * frac is the tensor-pipe utilisation; traffic = ncu dram bytes read + written per launch "
-                            "(committed single-pass capture), algorithmic bytes = 805 MB",
+                            "1.5 * frac is the tensor-pipe utilisation; algorithmic bytes = 805 MB",
                     "kernel_ms": gemm_ms, "prep_ms_per_step": prof["prep_ms"] / prof_steps,
                     "step_frac": (2.0 * M * N * K / (ms_step * 1e-3) / 1e12) / tf32_peak if world == 1 else None}
 
@@ -424,7 +420,7 @@ def run_ours(args):
                                      "note": "three tf32 passes over hi/lo pieces: fp32-faithful without the row/column scaling of the default mode"}
         modes["tf32x1_fast_mode"] = {"tflops": 2.0 * M * N * K / ms1 / 1e9, "ms": ms1, "tolerance": "normwise 2e-3 (hardware truncates fp32 -> tf32)",
                                      "frac_of_tf32_peak": 2.0 * M * N * K / ms1 / 1e9 / (peaks["bf16"] / 2.0),
-                                     "note": "TMA reads the caller's fp32 memory directly: no preparation pass at all"}
+                                     "note": "TMA reads A directly; B (row-major = MN-major) is first gathered K-major, since wgmma reads tf32 tiles K-major only"}
         Ab = A.view(M, K).to(torch.bfloat16); Bb = B.view(K, N).to(torch.bfloat16); Cb = torch.empty(M, N, dtype=torch.bfloat16, device=dev)
         msb = timed(lambda: L.gemm_strided(M, N, K, 1.0, Ab, K, 1, Bb, N, 1, 0.0, Cb, N, 1), half, 2)
         modes["bf16_8192_config4"] = {"tflops": 2.0 * M * N * K / msb / 1e9, "ms": msb, "frac_of_bf16_peak": 2.0 * M * N * K / msb / 1e9 / peaks["bf16"]}
@@ -482,7 +478,7 @@ def run_ours(args):
                                    + ("" if world == 1 else "; row-sharded: total M=%d, B travels over NCCL from rank 0 every step (prepared fp16 pieces + scales, column panels) "
                                                             "(laser_b200_gemm_rowsharded_f32_dev)" % (M * world)),
                        "global_M": M * world, "N": N, "K": K, "parallelism": "rowshard%d" % world,
-                       "f32_mode": "f16x3 (fp32-faithful, default)", "l2": "inputs larger than L2 (A+B+C = 805 MB vs 126 MB)",
+                       "f32_mode": "f16x3 (fp32-faithful, default)", "l2": "inputs larger than L2 (A+B+C = 805 MB vs 50 MB on an H100)",
                        "timing": "CUDA events on the launching stream, barrier + synchronize both sides, max over ranks"},
             "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches), "roofline": roofline, "parity": parity,
             "strong_m32768": strong,
@@ -496,6 +492,21 @@ def run_ours(args):
         dist.destroy_process_group()
     if not ok:
         raise SystemExit("bench.py: PARITY FAILED (see the 'parity' / 'strong_m32768.parity' keys of the line)")
+
+
+DUMP_ROWS = 1024
+
+
+def dump_outputs(out_dir, C):
+    """a fixed sample of DUMP_ROWS rows of C (seeded, sorted; 32 MB of float32 at N = 8192) and their indices"""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    rows = np.sort(np.random.default_rng(20240).choice(C.shape[0], size=min(DUMP_ROWS, C.shape[0]), replace=False))
+    sample = C[torch.as_tensor(rows, device=C.device)].cpu().numpy().astype(np.float32)
+    np.save(os.path.join(out_dir, "c_rows.npy"), sample)
+    np.save(os.path.join(out_dir, "c_row_index.npy"), rows.astype(np.float64))
 
 
 def _finite_json(x):
@@ -546,7 +557,11 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded row sample of the last timed step's C (rank 0's panel) as .npy files into DIR")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU step's output; the reference arm has none (use --impl ours)")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
         run_reference(args)

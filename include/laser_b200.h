@@ -1,5 +1,5 @@
 /*
- * laser_b200.h -- C ABI of the B200-native strided GEMM that drops in for
+ * laser_b200.h -- C ABI of the H100-native strided GEMM that drops in for
  * mratsim/laser's `gemm_strided` hot path.
  *
  * Every entry point below states the reference interface it replaces
@@ -22,7 +22,7 @@
  * Return value: 0 on success, non-zero LASER_B200_E* otherwise;
  * laser_b200_last_error() gives a thread-local message.  The reference
  * returns void and validates nothing (gemm.nim:184-247); the Nim wrapper turns
- * non-zero into an exception.  There is NO CPU fallback: if no sm_100 device
+ * non-zero into an exception.  There is NO CPU fallback: if no sm_90 device
  * is usable every compute entry point fails with LASER_B200_ENODEVICE.
  */
 #ifndef LASER_B200_H
@@ -37,7 +37,7 @@ extern "C" {
 
 #define LASER_B200_OK 0
 #define LASER_B200_EINVAL 1     /* bad argument (negative size, null pointer) */
-#define LASER_B200_ENODEVICE 2  /* no usable sm_100 GPU / driver */
+#define LASER_B200_ENODEVICE 2  /* no usable sm_90 GPU / driver */
 #define LASER_B200_ECUDA 3      /* CUDA runtime or driver error */
 #define LASER_B200_ENOMEM 4     /* device allocation failed */
 #define LASER_B200_EUNSUPPORTED 5
@@ -48,13 +48,14 @@ extern "C" {
  *       The reference's analogue of this choice is its run-time ISA dispatch, gemm.nim:228-247. */
 #define LASER_B200_PATH_AUTO 0
 #define LASER_B200_PATH_SIMT 1    /* exact fp32 FFMA chain, bit-equal to the CPU reference order */
-#define LASER_B200_PATH_TF32X1 2  /* tcgen05 kind::tf32, one pass over the caller's memory (fast, ~1e-3 relative) */
-#define LASER_B200_PATH_TF32X3 3  /* tcgen05 kind::tf32, hi/lo split, three passes (fp32-faithful, any dynamic range) */
-#define LASER_B200_PATH_BF16 4    /* tcgen05 kind::f16 (bf16 inputs, fp32 accumulate)         */
+#define LASER_B200_PATH_TF32X1 2  /* wgmma tf32, one pass (fast, ~1e-3 relative); TMA reads K-major operands in place,
+                                   * an MN-major operand (e.g. a row-major B) is first gathered K-major */
+#define LASER_B200_PATH_TF32X3 3  /* wgmma tf32, hi/lo split, three passes (fp32-faithful, any dynamic range) */
+#define LASER_B200_PATH_BF16 4    /* wgmma bf16 (bf16 inputs, fp32 accumulate)                */
 /* 5 and 6 were round-1 modes (tf32 + bf16 correction terms; two bf16 pieces): superseded by F16X3, removed */
 #define LASER_B200_PATH_F16X3 7   /* DEFAULT fp32 mode.  Every row of A and column of B is scaled by its own power of two
                                    * (device-side abs-max along K, no host synchronisation) and split into two FP16 pieces
-                                   * (11 + 11 bits); three kind::f16 passes hi*lo', lo*hi', hi*hi' over tiles loaded once; the
+                                   * (11 + 11 bits); three wgmma f16 passes hi*lo', lo*hi', hi*hi' over tiles loaded once; the
                                    * epilogue undoes the scales.  1.5 tf32-equivalents per MAC; <= 3*2^-22 per product for
                                    * entries within 2^-17 of their row's / column's maximum, smaller entries keep an absolute
                                    * precision of 2^-39 of that maximum (the row/column-norm error model of a blocked GEMM) */

@@ -1,7 +1,7 @@
-"""laser_b200 -- B200-native (sm_100a) drop-in for mratsim/laser's strided GEMM hot path.
+"""laser_b200 -- H100-native (sm_90a) drop-in for mratsim/laser's strided GEMM hot path.
 
 The product is the C-ABI shared library laser_b200/lib/liblaser_b200.so (hand-written CUDA:
-tcgen05/TMEM/TMA tensor-core kernels + an exact SIMT kernel); this package is the thin
+wgmma/TMA tensor-core kernels + an exact SIMT kernel); this package is the thin
 host-side mirror of the reference interface on top of it.  See DESIGN.md / INTEGRATION.md.
 """
 from ._capi import (PATH_AUTO, PATH_BF16, PATH_F16X3, PATH_NAMES, PATH_SIMT, PATH_TF32X1, PATH_TF32X3, LaserB200Error, lib,

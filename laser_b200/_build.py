@@ -1,6 +1,6 @@
-"""Builds laser_b200/lib/liblaser_b200.so with nvcc for sm_100a (in-tree, no JIT cache).
+"""Builds laser_b200/lib/liblaser_b200.so with nvcc for sm_90a (in-tree, no JIT cache).
 
-One object per translation unit, compiled in parallel (the tcgen05 kernel families are the slow ones), then one link."""
+One object per translation unit, compiled in parallel (the wgmma kernel families are the slow ones), then one link."""
 import concurrent.futures
 import fcntl
 import hashlib
@@ -20,12 +20,12 @@ HEADERS = ["ptx.cuh", "f16_scale.cuh", "gemm_tc.cuh", "tc_params.h", "tc_launch.
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",   # NOT -arch=sm_100a: tcgen05 needs the 'a' PTX target
+    "-gencode", "arch=compute_90a,code=sm_90a",   # the 'a' target: wgmma and setmaxnreg exist only in sm_90a
     "-lineinfo",
     "-Xcompiler", "-fPIC",
 ]
 LINK_FLAGS = ["-shared", "-cudart", "static",       # no libcuda/libcudart link dependency: loads on CPU-only hosts
-              "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-ldl"]
+              "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-ldl"]
 
 
 def _nvcc():

@@ -2,10 +2,10 @@
 //
 // Mirrors the host half of the reference's gemm_strided (gemm.nim:184-247): build the
 // three matrix views, pick a kernel family (the reference picks an ISA micro-kernel at
-// run time, gemm.nim:228-247; here: exact SIMT vs tcgen05), prepare the operands
+// run time, gemm.nim:228-247; here: exact SIMT vs wgmma), prepare the operands
 // (the reference allocates packing Tiles per call, gemm_tiling.nim:312-341; here: TMA
 // tensor maps, plus the two-piece workspace of the fp32-faithful modes) and launch.
-// The tcgen05 kernels live in their own translation units (tc_*.cu, tc_launch.h).
+// The wgmma kernels live in their own translation units (tc_*.cu, tc_launch.h).
 // There is no CPU fallback anywhere in this file.
 #include "../../include/laser_b200.h"
 
@@ -100,17 +100,18 @@ struct Ctx {
   int map_cache_next = 0;
   int raster_g = 0;       // env LASER_B200_RASTER (0 = default)
   bool splitk_enabled = true;  // env LASER_B200_SPLITK=0 disables split-K
-  bool c_tma = true;           // env LASER_B200_C_TMA=0: the tensor-core epilogue stores C with plain 16-byte stores
   bool f64_dmma = true;        // env LASER_B200_F64_DMMA=0: fp64 problems stay on the CUDA-core kernel
   bool prep_ring = true;       // env LASER_B200_PREP_RING=0: register-only preparation kernel for K-major operands
   bool ring_attr_set = false, dmma_attr_set = false;
   int64_t panel_rows = 1024;  // env LASER_B200_PANEL_ROWS: row-panel height of the pipelined host-pointer entry
   bool panel_taper = false;   // env LASER_B200_PANEL_TAPER=1: cut the last row panel finer (shorter PCIe tail)
-  bool cta_pair = true;   // env LASER_B200_CTA_PAIR=0 forces the single-CTA kernel
-  // K extent per TMEM accumulation block of the fp32-faithful modes (env LASER_B200_KC).  Measured on the round-2 kernel at
-  // 8192^3 (profiles/r02_kc_sweep.md): 128 -> 2.147 ms, 256 -> 2.111 ms, 512 -> 2.044 ms, while the truncation bias of the
-  // tensor core's accumulator doubles with every step (mean_relative_error on U(-0.1,0.1): 3.4e-6 / 6.5e-6 / 1.2e-5 against the
-  // reference's 1e-5 gate): 128 keeps a 3x margin for 1.7 % of the time
+  // env LASER_B200_CTA_PAIR=1: clusters of two CTAs on neighbouring 128-row blocks of one B panel, sharing one tile
+  // scheduler.  Off by default: each CTA still loads its own B tile, and in alternated runs at 8192^3 the pairing was 3-4 %
+  // faster on an H100 SXM at 700 W but 5 % slower on one at 400 W
+  bool cta_pair = false;
+  // K extent per accumulator block of the fp32-faithful modes (env LASER_B200_KC): the tensor core's own accumulation does
+  // not round to nearest, and its bias grows with the chain it accumulates; after each block the sums are added to fp32
+  // running sums with round-to-nearest.  Shorter blocks cost a few register additions per k-tile.
   int kc_faithful = 128;
   bool dyn_sched = true;  // env LASER_B200_DYNSCHED=0: static round-robin tiles instead of the atomic counter
   bool pdl = true;        // env LASER_B200_PDL=0: ordinary launch of the GEMM kernel after the preparation kernels
@@ -165,9 +166,9 @@ int get_ctx(Ctx **out) {
     if (!c.ready) {
       cudaDeviceProp prop;
       CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-      if (prop.major != 10)
+      if (prop.major != 9 || prop.minor != 0)
         return set_error(LASER_B200_ENODEVICE,
-                         "device %d is sm_%d%d; this library is built for sm_100a only (no fallback)",
+                         "device %d is sm_%d%d; this library is built for sm_90a only (no fallback)",
                          dev, prop.major, prop.minor);
       c.dev = dev;
       c.sm_count = prop.multiProcessorCount;
@@ -193,7 +194,6 @@ int get_ctx(Ctx **out) {
       if (const char *sk = getenv("LASER_B200_SPLITK")) c.splitk_enabled = atoi(sk) != 0;
       if (const char *pr = getenv("LASER_B200_PREP_RING")) c.prep_ring = atoi(pr) != 0;
       if (const char *dm = getenv("LASER_B200_F64_DMMA")) c.f64_dmma = atoi(dm) != 0;
-      if (const char *ct = getenv("LASER_B200_C_TMA")) c.c_tma = atoi(ct) != 0;
       if (const char *pt = getenv("LASER_B200_PANEL_TAPER")) c.panel_taper = atoi(pt) != 0;
       if (const char *ds = getenv("LASER_B200_DYNSCHED")) c.dyn_sched = atoi(ds) != 0;
       if (const char *pd = getenv("LASER_B200_PDL")) c.pdl = atoi(pd) != 0;
@@ -503,7 +503,9 @@ template <int ESZ>
 int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w, int block_mn,
                     OperandMaps *m, bool *used_ws, cudaStream_t s) {
   using ET = typename std::conditional<ESZ == 4, float, uint16_t>::type;
-  const Major mj = classify(o, ESZ);
+  // wgmma reads tf32 tiles K-major only: an MN-major fp32 operand of the tf32 modes is gathered into compact K-major rows
+  const Major mj0 = classify(o, ESZ);
+  const Major mj = (ESZ == 4 && mode != SPLIT_F16X2 && mj0 == MN_MAJOR) ? GENERAL : mj0;
   const int64_t vec = 16 / ESZ;
   int rc;
   if (mj != GENERAL && mode == SPLIT_NONE) {
@@ -616,16 +618,6 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
   p.M = M; p.N = N; p.K = K; p.alpha = alpha; p.beta = beta;
   p.C = C; p.rsC = rsC; p.csC = csC; p.zero = 0; p.epi = epi;
   if (f16) { p.amax_a = f16->a; p.amax_b = f16->b; }
-  std::memset(&l.c, 0, sizeof l.c);
-  if constexpr (std::is_same<OutT, float>::value) {
-    // C leaves through TMA (smem-staged cp.async.bulk.tensor stores of 32 x 32 boxes) when the copy engine can address it:
-    // unit column stride, 16-byte aligned base and row pitch (LASER_B200_C_TMA=0: plain 16-byte stores)
-    if (c.c_tma && csC == 1 && rsC >= N && (rsC * 4) % 16 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0 && N >= 32 && M >= 1) {
-      const int rc_map = encode_map(c, &l.c, 4, C, N, M, rsC, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B);
-      if (rc_map) return rc_map;
-      p.c_tma = 1;
-    }
-  }
   const int npass = (kind == TC_TF32X3 || kind == TC_F16X3) ? 3 : 1;
   const TcPlanCfg cfg{c.kc_faithful, c.raster_g, c.splitk_enabled, c.sm_count};
   if (kind == TC_BF16 || kind == TC_F16X3) tc_plan<2, std::is_same<OutT, float>::value>(p, npass, pair, cfg);
@@ -703,10 +695,10 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   if (mode == SPLIT_F16X2 && (rc = f16_scales(c, M, N, &f16_b_off))) { prof_abort(c, &ep); return rc; }
   rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s);
   if (rc) { prof_abort(c, &ep); return rc; }
-  // CTA pairs (cta_group::2, 256 x 256 tiles) whenever there are at least two 128-row blocks
+  // clusters of two CTAs (256 x 128 tiles) when enabled and there are at least two 128-row blocks
   const bool pair = c.cta_pair && M > TC_BLOCK_M;
   if (b_ready) CUDA_TRY(cudaStreamWaitEvent(s, b_ready, 0));
-  rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), pair ? TC_BLOCK_N / 2 : TC_BLOCK_N, &mb, &used_ws, s);
+  rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, s);
   if (rc) { prof_abort(c, &ep); return rc; }
   const int prep_launches = static_cast<int>(g_launches.load() - launches_before);
   rc = prof_close(c, s, &ep, prep_launches);
@@ -835,7 +827,7 @@ int gemm_packed_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A
       if ((rc = prof_close(c, s, &ep, prep_launches))) return rc;
       f16.a = static_cast<const uint32_t *>(c.f16s.ptr);
     }
-    if ((rc = packed_maps(c, packedB, N, K, pair ? TC_BLOCK_N / 2 : TC_BLOCK_N, &mb, &f16.b))) return rc;
+    if ((rc = packed_maps(c, packedB, N, K, TC_BLOCK_N, &mb, &f16.b))) return rc;
     if ((rc = tc_run<float>(c, TC_F16X3, M, N, K, alpha, ma, mb, beta, C, rsC, csC, pair, s, Epilogue(), &f16,
                             prep_launches > 0 && !c.profiling)))
       return rc;
@@ -1081,7 +1073,7 @@ int host_gemm_f32_pipelined(Ctx &c, int64_t M, int64_t N, int64_t K, float alpha
   Operand ob{dB, N, K, csB, rsB};
   int64_t f16_b_off = 0;       // f16x3: room for the longest panel's rows of A + the columns of B
   if (f16x3 && (rc = f16_scales(c, panel_rows < M ? panel_rows : M, N, &f16_b_off))) return rc;
-  if ((rc = prepare_operand<4>(c, ob, mode, ws_of_B(c, f16_b_off), pair ? TC_BLOCK_N / 2 : TC_BLOCK_N, &mb, &used_ws, cmp)))
+  if ((rc = prepare_operand<4>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, cmp)))
     return rc;
   const F16Scales f16{static_cast<const uint32_t *>(c.f16s.ptr), static_cast<const uint32_t *>(c.f16s.ptr) + f16_b_off};
   // ---- row panels ----

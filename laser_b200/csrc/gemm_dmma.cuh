@@ -4,9 +4,9 @@
 // every C[i,j] is the k-sequential FMA chain from 0 inside blocks of kc = 2048 / sizeof(double) = 256 (gemm_tiling.nim:
 // 309-310), followed per block by the reference epilogue on C itself with beta' = beta on the first block and 1 afterwards
 // (gemm.nim:150-158, gemm_ukernel_generic.nim:53-76).  One DMMA computes, per output element, four steps of exactly that
-// chain (d = fma(a_k, b_k, d) for k = 0..3 in order -- checked bit for bit against the oracle on the B200,
-// tests/test_gpu_parity.py::test_f64_dmma_bit_exact), so the tensor core only changes who executes the chain.  tcgen05 has
-// no fp64 kind; mma.sync is the one tensor path the part offers for doubles (gemm.nim:234-246 dispatches float64 to the
+// chain (d = fma(a_k, b_k, d) for k = 0..3 in order -- checked bit for bit against the oracle by
+// tests/test_gpu_parity.py::test_f64_dmma_bit_exact), so the tensor core only changes who executes the chain.  wgmma has
+// no fp64 type; mma.sync is the one tensor path the part offers for doubles (gemm.nim:234-246 dispatches float64 to the
 // same loop nest as float32: this is that row of the dispatch).
 //
 // Tiling: 128 x 128 x 16 block tile, 256 threads = 8 warps in a 4 (m) x 2 (n) grid, warp tile 32 x 64 = 4 x 8 DMMA tiles

@@ -1,4 +1,4 @@
-// gemm_tc.cuh -- the tcgen05 / TMEM / TMA strided GEMM for sm_100a (ONE kernel template, round 2).
+// gemm_tc.cuh -- the wgmma / TMA strided GEMM for sm_90a (ONE kernel template).
 //
 // What it replaces in the reference (mratsim/laser, paths relative to
 // laser/primitives/matrix_multiplication/):
@@ -6,39 +6,37 @@
 //       copy engine resolves the operand's strides and lands 128-byte-swizzled
 //       tiles in shared memory; no packing buffers exist.
 //   gebb_ukernel register micro-kernel (gemm_ukernel_generator.nim:140-250)
-//       -> tcgen05.mma (kind::tf32 / kind::f16) issued by ONE thread per CTA pair,
-//       accumulators in TMEM (128 lanes x 256 columns fp32 per tile and CTA).
+//       -> wgmma.mma_async (tf32 / f16 / bf16) issued by two consumer warpgroups per CTA, each
+//       owning 64 rows x 128 columns of the 128 x 128 output tile, accumulators in registers.
 //   gemm_impl loop pc (gemm.nim:150-158: K is cut in kc blocks, every block's partial
 //       product is ADDED to C in fp32) -> K is cut in accumulation blocks of `kb_per_block`
-//       k-tiles: the tensor core accumulates one block in TMEM, the epilogue warps drain
-//       it and add it (IEEE round-to-nearest FADD) to running sums held in registers
-//       while the tensor core is already working on the next block in the other TMEM
-//       stage.  This matters numerically: the tensor core's own accumulator truncates
-//       (measured on B200: ~0.3 ulp of bias per MMA instruction, i.e. 5.5e-5 relative at
-//       K = 8192 for positive inputs), so long chains must not live in TMEM.
+//       k-tiles: the tensor core accumulates one block in the wgmma accumulator registers, which
+//       are then added (IEEE round-to-nearest FADD) to running sums held in other registers.
+//       This matters numerically: the tensor core's own accumulation does not round to nearest,
+//       so long chains must not live in the accumulator.
 //   gebp_mkernel loops jr/ir + loop ic (gemm.nim:48-176; `omp for` over ic blocks)
-//       -> persistent CTAs (or CTA pairs, cta_group::2) that DRAW 128 x 256 (256 x 256) output
-//       tiles from an atomic counter in device memory (a scheduler thread per pair publishes the
-//       unit through shared memory / DSMEM): tiles go to whichever pair is free, so SMs that start
-//       late (another kernel -- e.g. the NCCL broadcast of the row-sharded driver -- still holds
-//       them) or run slower simply take fewer tiles.
+//       -> persistent CTAs (or clusters of two CTAs on neighbouring 128-row blocks of one
+//       256 x 128 tile) that DRAW output tiles from an atomic counter in device memory (a scheduler
+//       thread per cluster publishes the unit through shared memory / DSMEM): tiles go to whichever
+//       CTA is free, so SMs that start late (another kernel -- e.g. the NCCL broadcast of the
+//       row-sharded driver -- still holds them) or run slower simply take fewer tiles.
 //   epilogues (gemm_ukernel_generic.nim:53-126)
 //       -> alpha/beta in fp32 from the running sums; beta == 0 never reads C; optional fused
 //       bias + activation (the reference's TODO at gemm.nim:196).
+//
+// Warp roles (384 threads): warp 0 lane 0 issues the TMA loads into a ring of stages, warp 3 lane 0 of the
+// leader CTA runs the tile scheduler, warpgroups 1 and 2 issue the MMAs and store their rows of C.
 //
 // Template parameters:
 //   ESZ     element size of the tiles (4: fp32 containers read as tf32, 2: 16-bit)
 //   FMT16   ptx::kFmtBF16 or ptx::kFmtF16 (ESZ == 2)
 //   NPASS   1: one MMA pass over (A, B).  3: fp32-faithful product of two-piece operands
 //           x = hi + lo: per k-tile the stage holds FOUR tiles (A_hi, A_lo, B_hi, B_lo), each loaded
-//           ONCE, and feeds three passes hi*lo', lo*hi', hi*hi' (round 1 re-loaded hi for every pass:
-//           6 tile loads per k-tile; the L2 -> shared-memory path is the scarce resource of this
-//           kernel, ~6.3 KB/clk for the whole chip)
-//   A_MN/B_MN operand major-ness (UMMA reads K-major and MN-major tiles natively, so A^T*B,
-//           A*B^T ... need no data movement)
+//           ONCE, and feeds three passes hi*lo', lo*hi', hi*hi'
+//   A_MN/B_MN operand major-ness (wgmma reads K-major and MN-major 16-bit tiles natively, so A^T*B,
+//           A*B^T ... need no data movement; tf32 tiles must be K-major)
 //   OutT    float or uint16_t (bf16 bits)
-//   PAIR    clusters of 2 CTAs; CTA rank r owns rows [128r, 128r+128) of the 256-row tile and
-//           stages half of the B columns
+//   PAIR    clusters of 2 CTAs; CTA rank r owns rows [128r, 128r+128) of the 256-row tile
 //   SCALED  F16X3 mode: the operands are fp16 pieces of A's rows / B's columns scaled by powers of
 //           two (f16_scale.cuh); the epilogue multiplies output (i, j) by 2^-sA[i] * 2^-sB[j]
 #pragma once
@@ -51,8 +49,8 @@
 
 namespace lb200 {
 
-// (out of line: inlined into the 128 unrolled stores of each of the three store paths the tanhf / expf bodies made the kernel
-// 370 KB -- the epilogue warps then miss the 32 KB instruction cache on every tile)
+// (out of line: inlined into the unrolled stores the tanhf / expf bodies would multiply the kernel's code size, and the
+// consumer warps would miss the instruction cache on every tile)
 #ifndef LB200_HOST_EMULATION
 static __device__ __noinline__ float epi_act(float v, int act) {
 #else
@@ -79,13 +77,13 @@ template <int ESZ, uint32_t FMT16, int NPASS, bool A_MN, bool B_MN, typename Out
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                const __grid_constant__ CUtensorMap mapB0, const __grid_constant__ CUtensorMap mapB1,
-               const __grid_constant__ CUtensorMap mapC, const TcParams p) {
+               const TcParams p) {
   static_assert(NPASS == 1 || NPASS == 3, "one pass, or the three passes of a two-piece product");
+  static_assert(ESZ == 2 || (!A_MN && !B_MN), "wgmma reads tf32 operands K-major only (capi.cu transposes MN-major fp32)");
   using Cfg = TcCfg<NPASS, PAIR>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int BLOCK_K = TC_ROW_BYTES / ESZ;             // 32 or 64 k-elements per k-tile
   constexpr int TILE_M = PAIR ? 2 * TC_BLOCK_M : TC_BLOCK_M;  // rows of one scheduled tile
-  constexpr uint32_t FMT = (ESZ == 4) ? ptx::kFmtTF32 : FMT16;
   const uint32_t cta_rank = PAIR ? ptx::cluster_ctarank() : 0u;
   const int sched_id = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
   const int sched_stride = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
@@ -93,16 +91,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
   LB200_DYN_SMEM(uint8_t, smem_raw);
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                               ~static_cast<uintptr_t>(1023));
-  uint8_t *store_staging = smem + STAGES * Cfg::STAGE_BYTES;   // 4 KB per epilogue warp (1024-byte aligned: TMA swizzle atoms)
-  uint64_t *bars = reinterpret_cast<uint64_t *>(store_staging + Cfg::STORE_STAGING_BYTES);
+  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t *full_bar = bars;                        // [STAGES]
   uint64_t *empty_bar = bars + STAGES;              // [STAGES]
-  uint64_t *tmem_full = bars + 2 * STAGES;          // [TC_ACC_STAGES]
-  uint64_t *tmem_empty = tmem_full + TC_ACC_STAGES; // [TC_ACC_STAGES]
-  uint64_t *sched_full = tmem_empty + TC_ACC_STAGES;   // the scheduler published a unit (one slot)
-  uint64_t *sched_empty = sched_full + 1;              // every consumer of the pair has read it (leader's copy counts)
-  uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(sched_empty + 1);
-  int *sched_unit = reinterpret_cast<int *>(tmem_base_smem + 1);
+  uint64_t *sched_full = bars + 2 * STAGES;         // the scheduler published a unit (one slot)
+  uint64_t *sched_empty = sched_full + 1;           // every consumer of the pair has read it (leader's copy counts)
+  int *sched_unit = reinterpret_cast<int *>(sched_empty + 1);
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -123,8 +117,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
       kb_hi = min(num_kb, kb_lo + p.kb_per_split);
     }
   };
-  // consumers of the scheduler slot: producer thread of each CTA, the MMA thread, lane 0 of each epilogue warp
-  constexpr int SCHED_CONSUMERS = PAIR ? (2 + TC_EPI_WARPS) + (1 + TC_EPI_WARPS) : (2 + TC_EPI_WARPS);
+  // consumers of the scheduler slot: the producer thread and lane 0 of each consumer warp, in each CTA of the cluster
+  constexpr int SCHED_CONSUMERS = PAIR ? 2 * (1 + TC_EPI_WARPS) : (1 + TC_EPI_WARPS);
   // next unit of this pair, or -1.  One thread per consumer calls it; `ph` is that consumer's phase bit.
   auto next_unit = [&](uint32_t &ph) -> int {
     if constexpr (PAIR) ptx::mbar_wait_cluster(sched_full, ph);   // the slot of CTA 1 was written by CTA 0
@@ -145,40 +139,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
       ptx::prefetch_tensormap(&mapA1);
       ptx::prefetch_tensormap(&mapB1);
     }
-    if (p.c_tma) ptx::prefetch_tensormap(&mapC);
   }
   if (threadIdx.x == 32) {
     for (int i = 0; i < STAGES; ++i) {
-      // pair: the leader's full barrier takes its own arrive.expect_tx plus the peer's arrive
-      ptx::mbar_init(&full_bar[i], PAIR ? 2 : 1);
-      ptx::mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < TC_ACC_STAGES; ++i) {
-      ptx::mbar_init(&tmem_full[i], 1);
-      // pair: the epilogue threads of BOTH CTAs release the leader's accumulator stage
-      ptx::mbar_init(&tmem_empty[i], PAIR ? 2 * TC_EPI_THREADS : TC_EPI_THREADS);
+      ptx::mbar_init(&full_bar[i], 1);
+      ptx::mbar_init(&empty_bar[i], TC_EPI_WARPS);   // lane 0 of every consumer warp releases the stage
     }
     ptx::mbar_init(sched_full, 1);
     ptx::mbar_init(sched_empty, SCHED_CONSUMERS);
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    if constexpr (PAIR) ptx::tmem_alloc_pair<TC_TMEM_COLS>(tmem_base_smem);
-    else ptx::tmem_alloc<TC_TMEM_COLS>(tmem_base_smem);
-  }
-  ptx::tc_fence_before_sync();
-  __syncthreads();                          // CTA-level: barrier inits + TMEM base visible to all warps
+  __syncthreads();                          // CTA-level: barrier inits visible to all warps
   if constexpr (PAIR) ptx::cluster_sync();  // peer barriers must exist before any remote arrive
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_base_smem;
   // programmatic dependent launch: everything above overlapped the tail of the preceding kernel of the stream (the operand
   // preparation); its results (prepared tiles, abs-max words) are visible from here on.  No-op for an ordinary launch.
   ptx::griddep_wait();
 
   if (warp_idx < 4) {
-    ptx::setmaxnreg_dec<TC_REGS_CTRL>();  // hand registers to the epilogue warpgroups
+    ptx::setmaxnreg_dec<TC_REGS_CTRL>();  // hand registers to the consumer warpgroups
     if (warp_idx == 3 && lane == 0 && cta_rank == 0) {
-      // ===================== tile scheduler (one thread per pair) =====================
+      // ===================== tile scheduler (one thread per cluster) =====================
       uint32_t phase = 0;
       int next_static = sched_id;
       for (;;) {
@@ -199,7 +179,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
         ptx::mbar_arrive(sched_full);
         phase ^= 1u;
         if (u < 0) {
-          if (p.sched) {   // the last pair to run dry re-arms the counter for the next launch on this slot
+          if (p.sched) {   // the last cluster to run dry re-arms the counter for the next launch on this slot
             __threadfence();
             if (atomicAdd(p.sched + 1, 1u) == static_cast<unsigned int>(sched_stride - 1)) {
               p.sched[0] = 0u;
@@ -214,28 +194,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
       // ===================== TMA producer (one thread) =====================
       int stage = 0;
       uint32_t phase = 0, sched_phase = 0;
-      auto tma = [&](void *dst, const CUtensorMap *m, uint64_t *bar, int c0, int c1) {
-        if constexpr (PAIR) ptx::tma_load_2d_pair(dst, m, bar, c0, c1);  // bytes -> leader's barrier
-        else ptx::tma_load_2d(dst, m, bar, c0, c1);
-      };
       constexpr int MN_ATOM = TC_ROW_BYTES / ESZ;             // elements per 128-byte MN chunk
       constexpr int MN_BOX_BYTES = BLOCK_K * TC_ROW_BYTES;    // one [BLOCK_K][128 B] TMA box
       auto load_a = [&](uint8_t *dst, const CUtensorMap *m, uint64_t *bar, int m0, int k0) {
         if constexpr (!A_MN) {
-          tma(dst, m, bar, k0, m0);  // box {BLOCK_K, 128}
+          ptx::tma_load_2d(dst, m, bar, k0, m0);  // box {BLOCK_K, 128}
         } else {
 #pragma unroll
           for (int c = 0; c < TC_BLOCK_M / MN_ATOM; ++c)  // boxes {MN_ATOM, BLOCK_K}
-            tma(dst + c * MN_BOX_BYTES, m, bar, m0 + c * MN_ATOM, k0);
+            ptx::tma_load_2d(dst + c * MN_BOX_BYTES, m, bar, m0 + c * MN_ATOM, k0);
         }
       };
       auto load_b = [&](uint8_t *dst, const CUtensorMap *m, uint64_t *bar, int n0, int k0) {
         if constexpr (!B_MN) {
-          tma(dst, m, bar, k0, n0);  // box {BLOCK_K, B_COLS}
+          ptx::tma_load_2d(dst, m, bar, k0, n0);  // box {BLOCK_K, TC_BLOCK_N}
         } else {
 #pragma unroll
-          for (int c = 0; c < Cfg::B_COLS / MN_ATOM; ++c)
-            tma(dst + c * MN_BOX_BYTES, m, bar, n0 + c * MN_ATOM, k0);
+          for (int c = 0; c < TC_BLOCK_N / MN_ATOM; ++c)
+            ptx::tma_load_2d(dst + c * MN_BOX_BYTES, m, bar, n0 + c * MN_ATOM, k0);
         }
       };
       for (;;) {
@@ -244,17 +220,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
         int t, sp, mb, nb, kb_lo, kb_hi;
         decode_unit(u, t, sp, kb_lo, kb_hi);
         tile_coords(t, p.num_m_blocks, p.num_n_blocks, p.raster_g, mb, nb);
-        // pair: this CTA's 128 rows of A and its half of the B columns
+        // cluster: this CTA's 128 rows of A; both CTAs read the same B tile (neighbours in L2)
         const int m0 = mb * TILE_M + static_cast<int>(cta_rank) * TC_BLOCK_M;
-        const int n0 = nb * TC_BLOCK_N + static_cast<int>(cta_rank) * (TC_BLOCK_N - Cfg::B_COLS);
+        const int n0 = nb * TC_BLOCK_N;
         for (int kb = kb_lo; kb < kb_hi; ++kb) {
           ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          if constexpr (PAIR) {
-            if (cta_rank == 0) ptx::mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-            else ptx::mbar_arrive_leader(&full_bar[stage]);
-          } else {
-            ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          }
+          ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
           uint8_t *sa = smem + stage * Cfg::STAGE_BYTES;
           uint8_t *sb = sa + Cfg::A_STAGE_BYTES;
           const int k0 = kb * BLOCK_K;
@@ -265,81 +236,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
-    } else if (warp_idx == 1 && lane == 0 && cta_rank == 0) {
-      // ===================== MMA issuer (one thread; pair: the leader CTA only) =============
-      int stage = 0;
-      uint32_t phase = 0, sched_phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      constexpr int UMMA_K = 32 / ESZ;                        // 8 or 16 elements = 32 bytes
-      constexpr int K_STEPS = BLOCK_K / UMMA_K;               // 4
-      constexpr int MN_BOX_BYTES = BLOCK_K * TC_ROW_BYTES;
-      // MN-major 32-bit operands must use the 128B-swizzle-with-32B-atoms layout (4 k-rows per atom)
-      constexpr uint32_t MN_LAYOUT = ESZ == 4 ? ptx::kLayoutSw128Base32 : ptx::kLayoutSw128;
-      constexpr uint32_t MN_SBO = ESZ == 4 ? 512 : 1024;
-      constexpr uint32_t IDESC = ptx::make_idesc(FMT, A_MN ? 1 : 0, B_MN ? 1 : 0, TILE_M, TC_BLOCK_N);
-      for (;;) {
-        const int u = next_unit(sched_phase);
-        if (u < 0) break;
-        int t, sp, kb_lo, kb_hi;
-        decode_unit(u, t, sp, kb_lo, kb_hi);
-        for (int kb0 = kb_lo; kb0 < kb_hi; kb0 += p.kb_per_block) {
-          const int kb1 = min(kb_hi, kb0 + p.kb_per_block);
-          ptx::mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-          ptx::tc_fence_after_sync();
-          const uint32_t d_tmem = tmem_base + acc * TC_BLOCK_N;
-          bool fresh = true;  // next MMA overwrites the accumulator (start of an accumulation block)
-          for (int kb = kb0; kb < kb1; ++kb) {
-            ptx::mbar_wait(&full_bar[stage], phase);
-            ptx::tc_fence_after_sync();
-            const uint32_t a_addr = ptx::smem_u32(smem + stage * Cfg::STAGE_BYTES);
-            const uint32_t b_addr = a_addr + Cfg::A_STAGE_BYTES;
-            // three passes: the small cross terms hi*lo', lo*hi' first, then hi*hi'
-#pragma unroll
-            for (int pass = 0; pass < NPASS; ++pass) {
-              const uint32_t a_tile = a_addr + ((NPASS == 3 && pass == 1) ? TC_A_TILE_BYTES : 0);
-              const uint32_t b_tile = b_addr + ((NPASS == 3 && pass == 0) ? Cfg::B_TILE_BYTES : 0);
-#pragma unroll
-              for (int k = 0; k < K_STEPS; ++k) {
-                // K-major: step 32 bytes inside the 128-byte swizzle row.
-                // MN-major: step UMMA_K k-rows of 128 bytes.
-                const uint64_t ad =
-                    A_MN ? ptx::make_smem_desc(a_tile + k * UMMA_K * TC_ROW_BYTES, MN_BOX_BYTES, MN_SBO, MN_LAYOUT)
-                         : ptx::make_smem_desc(a_tile + k * 32, 0, 1024, ptx::kLayoutSw128);
-                const uint64_t bd =
-                    B_MN ? ptx::make_smem_desc(b_tile + k * UMMA_K * TC_ROW_BYTES, MN_BOX_BYTES, MN_SBO, MN_LAYOUT)
-                         : ptx::make_smem_desc(b_tile + k * 32, 0, 1024, ptx::kLayoutSw128);
-                const uint32_t accum = (fresh && pass == 0 && k == 0) ? 0u : 1u;
-                if constexpr (PAIR) {
-                  if constexpr (ESZ == 4) ptx::mma_tf32_ss_pair(d_tmem, ad, bd, IDESC, accum);
-                  else ptx::mma_f16_ss_pair(d_tmem, ad, bd, IDESC, accum);
-                } else {
-                  if constexpr (ESZ == 4) ptx::mma_tf32_ss(d_tmem, ad, bd, IDESC, accum);
-                  else ptx::mma_f16_ss(d_tmem, ad, bd, IDESC, accum);
-                }
-              }
-            }
-            fresh = false;
-            // frees the smem slot (in both CTAs of a pair) when these MMAs retire
-            if constexpr (PAIR) ptx::mma_commit_pair(&empty_bar[stage]);
-            else ptx::mma_commit(&empty_bar[stage]);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          // block complete -> the epilogue warps (of both CTAs) drain it
-          if constexpr (PAIR) ptx::mma_commit_pair(&tmem_full[acc]);
-          else ptx::mma_commit(&tmem_full[acc]);
-          if (++acc == TC_ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-        }
-      }
     }
   } else {
-    // ============ epilogue: 8 warps; warp w owns TMEM lanes 32*(w%4).. and 128 columns ============
+    // ============ consumers: warpgroup g = 0, 1 multiplies and stores rows [64 g, 64 g + 64) of the CTA's 128 ============
     ptx::setmaxnreg_inc<TC_REGS_EPI>();
-    const int q = warp_idx & 3;          // TMEM lane quarter this warp may read
-    const int h = (warp_idx - 4) >> 2;   // column half
-    int acc = 0;
-    uint32_t acc_phase = 0, sched_phase = 0;
-    const bool vec_ok_c = (p.csC == 1) && ((p.rsC * sizeof(OutT)) % 16 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+    const int g = (warp_idx - 4) >> 2;
+    const int wq = warp_idx & 3;          // warp of the warpgroup: rows 16 wq .. 16 wq + 15 of the warpgroup's 64
+    const int lr = lane >> 2;             // fragment row (and row + 8)
+    const int lc = 2 * (lane & 3);        // fragment column pair 8 i + lc, 8 i + lc + 1
+    constexpr int MMA_K = 32 / ESZ;                        // 8 (tf32) or 16 (16-bit) k-elements = 32 bytes per instruction
+    constexpr int K_STEPS = BLOCK_K / MMA_K;               // 4
+    constexpr int MN_BOX_BYTES = BLOCK_K * TC_ROW_BYTES;
+    // the warpgroup's 64 rows of A: 8 KB into the tile both for K-major (64 rows of 128 B) and MN-major (the second box)
+    constexpr uint32_t A_WG_BYTES = 64 * TC_ROW_BYTES;
+    int stage = 0;
+    uint32_t phase = 0, sched_phase = 0;
+    const bool vec_ok_c = (p.csC == 1) && ((p.rsC & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & (2 * sizeof(OutT) - 1)) == 0);
+    float acc[TC_ACC_REGS];
+#pragma unroll
+    for (int j = 0; j < TC_ACC_REGS; ++j) acc[j] = 0.0f;
     for (;;) {
       int u = 0;
       if (lane == 0) u = next_unit(sched_phase);
@@ -349,241 +264,136 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
       decode_unit(u, t, sp, kb_lo, kb_hi);
       tile_coords(t, p.num_m_blocks, p.num_n_blocks, p.raster_g, mb, nb);
       const int num_blocks = (kb_hi - kb_lo + p.kb_per_block - 1) / p.kb_per_block;  // accumulation blocks
-      const int64_t row = static_cast<int64_t>(mb) * TILE_M + cta_rank * TC_BLOCK_M + q * 32 + lane;   // of the product
-      const int64_t col0 = static_cast<int64_t>(nb) * TC_BLOCK_N + h * TC_EPI_COLS;
+      const int r_tile = static_cast<int>(cta_rank) * TC_BLOCK_M + 64 * g + 16 * wq + lr;   // first row, tile-local
+      const int64_t row0 = static_cast<int64_t>(mb) * TILE_M + r_tile;                      // of the product (+ 8: second)
+      const int64_t col0 = static_cast<int64_t>(nb) * TC_BLOCK_N + lc;                     // column of acc[4 i] is col0 + 8 i
       const bool split_unit = sp >= 0;
-      // SCALED: the abs-max words were written by earlier kernels of this stream.  The word of this thread's row of A and the
-      // words of B's 128 columns of this warp are fetched NOW, four per lane (lane l holds columns col0 + 4l .. 4l + 3), and
-      // handed out by warp shuffles when the tile is stored: fetching them per element at store time put a dependent global
-      // load in front of each of the 32 vector stores, ~13k cycles per tile during which the tensor core ran out of free
-      // accumulator stages (ncu source page, round 2).  Everything else the store needs is derived after the K loop, so
-      // that only these five words stay live next to the 128 running sums.
-      uint32_t amax_row = 0u, amax_col[4] = {0u, 0u, 0u, 0u};
+      // SCALED: the abs-max words were written by earlier kernels of this stream; this thread's two row words and 32 column
+      // words are fetched now and used only by the store after the K loop, so their latency hides behind the MMAs
+      uint32_t amax_row[2] = {0u, 0u}, amax_col[2 * TC_BLOCK_N / 8];
       if constexpr (SCALED) {
-        if (row < p.M) amax_row = p.amax_a[row];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int64_t c = col0 + 4 * lane + i;
-          if (c < p.N) amax_col[i] = p.amax_b[c];
+        for (int h = 0; h < 2; ++h)
+          if (row0 + 8 * h < p.M) amax_row[h] = p.amax_a[row0 + 8 * h];
+#pragma unroll
+        for (int j = 0; j < 2 * TC_BLOCK_N / 8; ++j) {
+          const int64_t c = col0 + 8 * (j >> 1) + (j & 1);
+          amax_col[j] = c < p.N ? p.amax_b[c] : 0u;
         }
       }
-      if (!split_unit && p.beta != 0.0f && row < p.M && col0 < p.N && p.csC == 1) {
-        // beta != 0: pull this thread's 512 bytes of old C into L2 now; they are needed only
-        // after the whole K loop of the tile, so the latency is free
-        const OutT *cp = reinterpret_cast<const OutT *>(p.C) + row * p.rsC + col0;
+      float run[TC_ACC_REGS];  // running sums of this thread's fragment (registers)
 #pragma unroll
-        for (int l = 0; l < TC_EPI_COLS * static_cast<int>(sizeof(OutT)) / 128; ++l) {
-          if (col0 + l * (128 / static_cast<int>(sizeof(OutT))) < p.N)
-            ptx::prefetch_l2(cp + l * (128 / sizeof(OutT)));
-        }
-      }
-      float run[TC_EPI_COLS];  // running sums of this thread's row segment (registers)
-#pragma unroll
-      for (int j = 0; j < TC_EPI_COLS; ++j) run[j] = 0.0f;
+      for (int j = 0; j < TC_ACC_REGS; ++j) run[j] = 0.0f;
       for (int blk = 0; blk < num_blocks; ++blk) {
-        ptx::mbar_wait(&tmem_full[acc], acc_phase);
-        ptx::tc_fence_after_sync();
-        const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * TC_BLOCK_N + h * TC_EPI_COLS;
-        // Eight 16-column chunks.  `dep` (always 0 at run time: p.zero is 0, but the compiler
-        // cannot know) makes the address of chunk c+1 depend on an addition of chunk c, so the
-        // scheduler cannot issue all eight loads first and keep 128 extra registers in flight.
-        uint32_t dep = 0;
+        const int kb0 = kb_lo + blk * p.kb_per_block;
+        const int kb1 = min(kb_hi, kb0 + p.kb_per_block);
+        int prev_stage = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          ptx::mbar_wait(&full_bar[stage], phase);
+          ptx::wgmma_fence();
+          const uint32_t a_addr = ptx::smem_u32(smem + stage * Cfg::STAGE_BYTES) + g * A_WG_BYTES;
+          const uint32_t b_addr = ptx::smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_STAGE_BYTES);
+          // three passes: the small cross terms hi*lo', lo*hi' first, then hi*hi'
 #pragma unroll
-        for (int c = 0; c < TC_EPI_COLS / 16; ++c) {
-          uint32_t r[16];
-          ptx::tmem_ld_32x32b_x16(t_addr + c * 16 + dep, r);
-          ptx::tmem_ld_wait(r);
+          for (int pass = 0; pass < NPASS; ++pass) {
+            const uint32_t a_tile = a_addr + ((NPASS == 3 && pass == 1) ? TC_A_TILE_BYTES : 0);
+            const uint32_t b_tile = b_addr + ((NPASS == 3 && pass == 0) ? Cfg::B_TILE_BYTES : 0);
 #pragma unroll
-          for (int j = 0; j < 16; ++j) run[c * 16 + j] = __fadd_rn(run[c * 16 + j], __uint_as_float(r[j]));
-          dep = (__float_as_uint(run[c * 16]) | __float_as_uint(run[c * 16 + 15])) & p.zero;
-        }
-        // this thread's TMEM reads of the block are done: hand the stage back to the MMA thread
-        ptx::tc_fence_before_sync();
-        if constexpr (PAIR) ptx::mbar_arrive_leader(&tmem_empty[acc]);
-        else ptx::mbar_arrive(&tmem_empty[acc]);
-        if (++acc == TC_ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-      }
-      // where this thread's 128 sums go.  Direct tile: its row of C, with alpha / beta / bias / activation.  Split unit: row
-      // (tile-local) of plane [sp][t - n_direct] of the workspace, raw (only the operand scales are undone).
-      OutT *crow_base;          // element (row, col0)
-      int64_t cs_u;             // column stride
-      int64_t ncols;            // columns of this thread's segment that exist
-      bool vec_ok;
-      float alpha_u, beta_u;
-      if (!split_unit) {
-        crow_base = reinterpret_cast<OutT *>(p.C) + (row < p.M ? row : 0) * p.rsC + col0 * p.csC;
-        cs_u = p.csC; ncols = p.N - col0; vec_ok = vec_ok_c; alpha_u = p.alpha; beta_u = p.beta;
-      } else {
-        const int64_t plane = static_cast<int64_t>(sp) * (num_tiles - p.n_direct) + (t - p.n_direct);
-        crow_base = reinterpret_cast<OutT *>(p.split_ws) +
-                    (plane * TILE_M + cta_rank * TC_BLOCK_M + q * 32 + lane) * TC_BLOCK_N + h * TC_EPI_COLS;
-        cs_u = 1; ncols = TC_EPI_COLS; vec_ok = true; alpha_u = 1.0f; beta_u = 0.0f;
-      }
-      const bool row_ok = row < p.M || split_unit;   // (rows past M of a split tile: zeros into the workspace)
-      float alpha_eff = alpha_u;
-      float cs[4] = {1.0f, 1.0f, 1.0f, 1.0f};
-      if constexpr (SCALED) {
-        alpha_eff = alpha_u * f16x2_unscale(amax_row);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) cs[i] = f16x2_unscale(amax_col[i]);
-      }
-      // factor of column col0 + j (j warp-uniform); every lane of the warp must call it
-      auto col_unscale = [&](int j) -> float {
-        if constexpr (SCALED) {
-          const float v = (j & 3) == 0 ? cs[0] : (j & 3) == 1 ? cs[1] : (j & 3) == 2 ? cs[2] : cs[3];
-          return __shfl_sync(0xffffffffu, v, j >> 2);
-        } else {
-          return 1.0f;
-        }
-      };
-      // ---- C <- alpha * sum + beta * C  (gemm_ukernel_generic.nim:53-76 semantics) ----
-      // control flow is warp-uniform down to the loads / stores themselves (col_unscale shuffles): only `row_ok` is per lane
-      if (col0 < p.N) {
-        const bool has_epi = !split_unit && ((p.epi.bias != nullptr) || (p.epi.act != 0));
-        const float row_bias = (has_epi && p.epi.bias && p.epi.bias_per_row && row_ok) ? p.epi.bias[row] : 0.0f;
-        if (vec_ok && ncols >= TC_EPI_COLS) {
-          if constexpr (sizeof(OutT) == 4) {
-            float4 *dst = reinterpret_cast<float4 *>(crow_base);
-            // Direct tiles of a TMA-addressable C leave through shared memory: the warp's 32 rows x 32 columns go, 128B-
-            // swizzled, into its 4 KB staging buffer and one cp.async.bulk.tensor store writes them as 32 full 128-byte
-            // lines (a plain 16-byte store per thread touches 32 different lines per warp instruction); the copy engine
-            // clips rows past M.  The buffer is reused once the previous store has READ it (wait_group.read).
-            const bool via_tma = p.c_tma != 0 && !split_unit;
-            uint8_t *stage_buf = store_staging + (warp_idx - 4) * 4096;
-            const int row_in_warp_tile = static_cast<int>(mb) * TILE_M + static_cast<int>(cta_rank) * TC_BLOCK_M + q * 32;
-            // batches of 4 x 16 B: with beta != 0 the four loads of a batch are in flight
-            // together (the old C lines were prefetched into L2 when the tile started)
-#pragma unroll
-            for (int b8 = 0; b8 < TC_EPI_COLS / 16; ++b8) {
-              float4 o[4];
-              if (beta_u != 0.0f && row_ok) {
-#pragma unroll
-                for (int e = 0; e < 4; ++e) o[e] = dst[b8 * 4 + e];
-              }
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int v4 = b8 * 4 + e;
-                float4 v;
-                v.x = alpha_eff * run[4 * v4 + 0];
-                v.y = alpha_eff * run[4 * v4 + 1];
-                v.z = alpha_eff * run[4 * v4 + 2];
-                v.w = alpha_eff * run[4 * v4 + 3];
-                if constexpr (SCALED) {
-                  v.x *= col_unscale(4 * v4 + 0);
-                  v.y *= col_unscale(4 * v4 + 1);
-                  v.z *= col_unscale(4 * v4 + 2);
-                  v.w *= col_unscale(4 * v4 + 3);
-                }
-                if (beta_u != 0.0f && row_ok) {
-                  v.x = fmaf(beta_u, o[e].x, v.x);
-                  v.y = fmaf(beta_u, o[e].y, v.y);
-                  v.z = fmaf(beta_u, o[e].z, v.z);
-                  v.w = fmaf(beta_u, o[e].w, v.w);
-                }
-                if (has_epi) {
-                  float4 bv = make_float4(row_bias, row_bias, row_bias, row_bias);
-                  if (p.epi.bias && !p.epi.bias_per_row) {
-                    const float *bp = p.epi.bias + col0 + 4 * v4;
-                    if ((reinterpret_cast<uintptr_t>(bp) & 15) == 0) bv = *reinterpret_cast<const float4 *>(bp);
-                    else bv = make_float4(bp[0], bp[1], bp[2], bp[3]);
-                  }
-                  v.x = epi_act(v.x + bv.x, p.epi.act);
-                  v.y = epi_act(v.y + bv.y, p.epi.act);
-                  v.z = epi_act(v.z + bv.z, p.epi.act);
-                  v.w = epi_act(v.w + bv.w, p.epi.act);
-                }
-                if (via_tma) {   // the finished values replace the sums they came from until the chunk is complete
-                  run[4 * v4 + 0] = v.x; run[4 * v4 + 1] = v.y; run[4 * v4 + 2] = v.z; run[4 * v4 + 3] = v.w;
-                } else if (row_ok) {
-                  dst[v4] = v;
-                }
-              }
-              if (via_tma && (b8 & 1) == 1) {   // 32 columns finished: stage them and hand them to the copy engine
-                // (the arithmetic above ran while the previous store was still reading the staging buffer)
-                if (lane == 0) ptx::tma_store_wait_read<0>();
-                __syncwarp();
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {   // 16-byte chunk j of this thread's 128-byte staging row
-                  const int v4 = (b8 - 1) * 4 + j;
-                  *reinterpret_cast<float4 *>(stage_buf + lane * 128 + ptx::sw128_chunk(lane, j) * 16) =
-                      make_float4(run[4 * v4 + 0], run[4 * v4 + 1], run[4 * v4 + 2], run[4 * v4 + 3]);
-                }
-                ptx::fence_proxy_async_smem();  // the generic-proxy writes above become visible to the async proxy
-                __syncwarp();
-                if (lane == 0) {
-                  ptx::tma_store_2d(&mapC, stage_buf, static_cast<int>(col0) + (b8 >> 1) * 32, row_in_warp_tile);
-                  ptx::tma_store_commit();
-                }
-              }
-            }
-          } else {
-            uint4 *dst = reinterpret_cast<uint4 *>(crow_base);
-#pragma unroll
-            for (int v8 = 0; v8 < TC_EPI_COLS / 8; ++v8) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = alpha_eff * run[8 * v8 + e] * col_unscale(8 * v8 + e);
-              if (beta_u != 0.0f && row_ok) {
-                const uint4 o = dst[v8];
-                const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  f[2 * e] = fmaf(beta_u, bf16_bits_to_f32(static_cast<uint16_t>(ow[e] & 0xffff)), f[2 * e]);
-                  f[2 * e + 1] = fmaf(beta_u, bf16_bits_to_f32(static_cast<uint16_t>(ow[e] >> 16)), f[2 * e + 1]);
-                }
-              }
-              if (has_epi) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                  const float bv = (p.epi.bias && !p.epi.bias_per_row) ? p.epi.bias[col0 + 8 * v8 + e] : row_bias;
-                  f[e] = epi_act(f[e] + bv, p.epi.act);
-                }
-              }
-              uint4 w;
-              w.x = f32_to_bf16_bits(f[0]) | (static_cast<uint32_t>(f32_to_bf16_bits(f[1])) << 16);
-              w.y = f32_to_bf16_bits(f[2]) | (static_cast<uint32_t>(f32_to_bf16_bits(f[3])) << 16);
-              w.z = f32_to_bf16_bits(f[4]) | (static_cast<uint32_t>(f32_to_bf16_bits(f[5])) << 16);
-              w.w = f32_to_bf16_bits(f[6]) | (static_cast<uint32_t>(f32_to_bf16_bits(f[7])) << 16);
-              if (row_ok) dst[v8] = w;
+            for (int k = 0; k < K_STEPS; ++k) {
+              // K-major: step 32 bytes inside the 128-byte swizzle row.  MN-major: step MMA_K k-rows of 128 bytes.
+              const uint64_t ad = A_MN ? ptx::make_smem_desc(a_tile + k * MMA_K * TC_ROW_BYTES, MN_BOX_BYTES, 1024, ptx::kLayoutSw128)
+                                       : ptx::make_smem_desc(a_tile + k * 32, 0, 1024, ptx::kLayoutSw128);
+              const uint64_t bd = B_MN ? ptx::make_smem_desc(b_tile + k * MMA_K * TC_ROW_BYTES, MN_BOX_BYTES, 1024, ptx::kLayoutSw128)
+                                       : ptx::make_smem_desc(b_tile + k * 32, 0, 1024, ptx::kLayoutSw128);
+              const uint32_t accum = (kb == kb0 && pass == 0 && k == 0) ? 0u : 1u;
+              if constexpr (ESZ == 4) ptx::wgmma_m64n128k8_tf32(acc, ad, bd, accum);
+              else if constexpr (FMT16 == ptx::kFmtF16) ptx::wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd, accum);
+              else ptx::wgmma_m64n128k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd, accum);
             }
           }
-        } else {
-          // any C strides / ragged right edge: scalar, predicated; one running pointer so
-          // that the unrolled loop does not keep 128 addresses live
-          OutT *dst = crow_base;
+          ptx::wgmma_commit();
+          // at most this k-tile's group still runs: the previous k-tile's stage goes back to the producer
+          ptx::wgmma_wait<1>();
+          if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev_stage]);
+          prev_stage = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        ptx::wgmma_wait<0>();
+        ptx::wgmma_hold(acc);
+        if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev_stage]);
+        // block complete: added (IEEE round-to-nearest) to the running sums, see the top of this file
 #pragma unroll
-          for (int j = 0; j < TC_EPI_COLS; ++j) {
-            float v = alpha_eff * run[j];
-            if constexpr (SCALED) v *= col_unscale(j);
-            if (j < ncols && row_ok) {
-              if (beta_u != 0.0f) {
-                if constexpr (sizeof(OutT) == 4) v = fmaf(beta_u, *dst, v);
-                else v = fmaf(beta_u, bf16_bits_to_f32(*dst), v);
-              }
-              if (has_epi) {
-                const float bv = (p.epi.bias && !p.epi.bias_per_row) ? p.epi.bias[col0 + j] : row_bias;
-                v = epi_act(v + bv, p.epi.act);
-              }
-              if constexpr (sizeof(OutT) == 4) *dst = v;
-              else *dst = f32_to_bf16_bits(v);
+        for (int j = 0; j < TC_ACC_REGS; ++j) run[j] = __fadd_rn(run[j], acc[j]);
+      }
+      // where this thread's sums go.  Direct tile: C, with alpha / beta / bias / activation.  Split unit: plane
+      // [sp][t - n_direct] of the workspace, tile-local rows / columns, raw (only the operand scales are undone).
+      float alpha_r[2] = {split_unit ? 1.0f : p.alpha, split_unit ? 1.0f : p.alpha};
+      if constexpr (SCALED) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) alpha_r[h] *= f16x2_unscale(amax_row[h]);
+      }
+      const float beta_u = split_unit ? 0.0f : p.beta;
+      const bool has_epi = !split_unit && ((p.epi.bias != nullptr) || (p.epi.act != 0));
+      float *ws_base = nullptr;
+      if (split_unit) {
+        const int64_t plane = static_cast<int64_t>(sp) * (num_tiles - p.n_direct) + (t - p.n_direct);
+        ws_base = p.split_ws + (plane * TILE_M + r_tile) * TC_BLOCK_N + lc;
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = row0 + 8 * h;
+        if (!split_unit && row >= p.M) continue;
+        const float row_bias = (has_epi && p.epi.bias && p.epi.bias_per_row) ? p.epi.bias[row] : 0.0f;
+        OutT *crow = split_unit ? nullptr : reinterpret_cast<OutT *>(p.C) + row * p.rsC;
+#pragma unroll
+        for (int i = 0; i < TC_BLOCK_N / 8; ++i) {
+          float v[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            v[e] = alpha_r[h] * run[4 * i + 2 * h + e];
+            if constexpr (SCALED) v[e] *= f16x2_unscale(amax_col[2 * i + e]);
+          }
+          if (split_unit) {   // (rows past M: zeros into the workspace)
+            *reinterpret_cast<float2 *>(ws_base + 8 * h * TC_BLOCK_N + 8 * i) = make_float2(v[0], v[1]);
+            continue;
+          }
+          const int64_t c = col0 + 8 * i;
+          if (c >= p.N) continue;
+          const bool pair_ok = vec_ok_c && c + 1 < p.N;
+          OutT *dst = crow + c * p.csC;
+          if (beta_u != 0.0f) {
+            float o[2] = {0.0f, 0.0f};
+            if constexpr (sizeof(OutT) == 4) {
+              if (pair_ok) { const float2 w = *reinterpret_cast<const float2 *>(dst); o[0] = w.x; o[1] = w.y; }
+              else { o[0] = dst[0]; if (c + 1 < p.N) o[1] = dst[p.csC]; }
+            } else {
+              o[0] = bf16_bits_to_f32(dst[0]);
+              if (c + 1 < p.N) o[1] = bf16_bits_to_f32(dst[pair_ok ? 1 : p.csC]);
             }
-            dst += cs_u;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) v[e] = fmaf(beta_u, o[e], v[e]);
+          }
+          if (has_epi) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float bv = (p.epi.bias && !p.epi.bias_per_row) ? (c + e < p.N ? p.epi.bias[c + e] : 0.0f) : row_bias;
+              v[e] = epi_act(v[e] + bv, p.epi.act);
+            }
+          }
+          if constexpr (sizeof(OutT) == 4) {
+            if (pair_ok) *reinterpret_cast<float2 *>(dst) = make_float2(v[0], v[1]);
+            else { dst[0] = v[0]; if (c + 1 < p.N) dst[p.csC] = v[1]; }
+          } else {
+            if (pair_ok) *reinterpret_cast<uint32_t *>(dst) = f32_to_bf16_bits(v[0]) | (static_cast<uint32_t>(f32_to_bf16_bits(v[1])) << 16);
+            else { dst[0] = f32_to_bf16_bits(v[0]); if (c + 1 < p.N) dst[p.csC] = f32_to_bf16_bits(v[1]); }
           }
         }
       }
     }
   }
 
-  if (warp_idx >= 4 && lane == 0) ptx::tma_store_wait<0>();   // the tile stores of this warp have left shared memory and landed
-  __syncwarp();
-  ptx::tc_fence_before_sync();
-  if constexpr (PAIR) ptx::cluster_sync();  // neither CTA may leave while its peer still uses its smem/TMEM
+  if constexpr (PAIR) ptx::cluster_sync();  // neither CTA may leave while its peer can still arrive on its barriers
   else __syncthreads();
-  ptx::tc_fence_after_sync();
-  if (warp_idx == 2) {
-    if constexpr (PAIR) ptx::tmem_dealloc_pair<TC_TMEM_COLS>(tmem_base);
-    else ptx::tmem_dealloc<TC_TMEM_COLS>(tmem_base);
-  }
 }
 
 }  // namespace lb200

@@ -1,7 +1,6 @@
-// ptx.cuh -- thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / fences) and the UMMA shared-memory and
-// instruction descriptors.  Hand-written; bit layouts follow the PTX ISA 8.6
-// tcgen05 chapter (cross-checked against cuda/__ptx and cute/arch/mma_sm100_desc.hpp).
+// ptx.cuh -- thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), clusters,
+// wgmma (fence / mma_async / commit / wait) and the wgmma shared-memory matrix descriptor.
+// Hand-written; bit layouts follow the PTX ISA "asynchronous warpgroup level matrix" chapter.
 #pragma once
 
 #include <cuda.h>
@@ -9,7 +8,7 @@
 #include <stdint.h>
 
 #ifdef LB200_HOST_EMULATION
-// tests/emu: the same names backed by a functional model of mbarrier / TMA / tcgen05 / TMEM on
+// tests/emu: the same names backed by a functional model of mbarrier / TMA / wgmma / clusters on
 // host threads (test infrastructure; see tests/emu/ptx_emu.h)
 #include "ptx_emu.h"
 #else
@@ -105,27 +104,6 @@ __device__ __forceinline__ void bulk_load_1d(void *smem_dst, const void *gsrc, u
                ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// position of 16-byte chunk j of row `row` inside a 128B-swizzled tile of 128-byte rows (what TMA expects to find / leaves)
-__device__ __forceinline__ int sw128_chunk(int row, int j) { return j ^ (row & 7); }
-// 2-D tiled store shared -> global (bulk async group).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *smem_src,
-                                             int32_t c0, int32_t c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() {
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
 __device__ __forceinline__ void prefetch_l2(const void *p) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
@@ -138,102 +116,85 @@ __device__ __forceinline__ void setmaxnreg_dec() {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
 
-// ------------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// ------------------------------------------------------------------- wgmma
+// All 128 threads of a warpgroup execute these together (.sync.aligned).  fence: the accumulator registers and the
+// shared-memory operands written before it are ordered before the following wgmma.mma_async; commit closes a group of
+// issued MMAs; wait<N> returns once at most N groups of this warpgroup are still pending (their accumulators are then valid
+// and their shared-memory operands may be overwritten).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers are threaded through an empty asm so that no use of them moves above a wgmma_wait
+__device__ __forceinline__ void wgmma_hold(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// Whole warp.  Writes the TMEM base address of `ncols` columns to *smem_dst.
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_dst) {
-  static_assert(NCOLS >= 32 && NCOLS <= 512 && (NCOLS & (NCOLS - 1)) == 0, "power of two >= 32");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-               ::"r"(smem_u32(smem_dst)), "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc];  one thread issues for the CTA.
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                            uint32_t idesc, uint32_t accumulate) {
+// D (64 x 128, fp32, registers of the warpgroup) (+)= A (64 x K, shared memory) * B (K x 128, shared memory).
+// scale_d == 0: D is overwritten.  TA / TB: 1 = the operand is MN-major (16-bit formats only; tf32 must be K-major).
+// Accumulator fragment: thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and, for i < 16, columns
+// 8 i + 2 (t % 4) + {0, 1}: d[4 i + {0, 1}] on the first row, d[4 i + {2, 3}] on the second.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t"
       "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                           uint32_t idesc, uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t"
       "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// mbarrier arrives once all tcgen05.mma issued so far by this thread complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-               ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread
-// (thread t of the warp reads lane base+t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, "
-      "%12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, "
-      "%30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, "
-      "%12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]),
-                 "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]),
-                 "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
-// tcgen05.ld is asynchronous: the destination registers are only valid after
-// tcgen05.wait::ld.  The registers are threaded through the wait as "+r" operands so
-// that the compiler cannot schedule any use of them above it.
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
 
-// ------------------------------------------------------------ CTA pairs (cta_group::2)
+// ------------------------------------------------------------ clusters of two CTAs
 // In a cluster launch the shared-window address of a CTA's own shared memory carries the
 // CTA's rank in bit 24; clearing it names the same offset in the even (leader) CTA of a pair.
 constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
@@ -290,97 +251,27 @@ __device__ __forceinline__ void st_shared_cluster_s32(int *p, uint32_t rank, int
 // the kernel was launched without the attribute); launch_dependents lets the next kernel of the stream start its prologue
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-// TMA load into THIS CTA's shared memory, transaction bytes credited to the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_2d_pair(void *smem_dst, const CUtensorMap *map, uint64_t *bar,
-                                                 int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)),
-        "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t *smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-               ::"r"(smem_u32(smem_dst)), "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-// D[tmem of both CTAs] (+)= A (128 rows from each CTA) * B (N/2 columns from each CTA)
-__device__ __forceinline__ void mma_tf32_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_f16_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                                uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit: the mbarrier at this offset in BOTH CTAs of the pair receives one arrival
-__device__ __forceinline__ void mma_commit_pair(uint64_t *bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-
 // ------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor (64 bit):
-//   [0,14)  start address >> 4          [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4 [46,48) version = 1 (Blackwell)
-//   [49,52) base offset = 0             [61,64) layout: 0 none, 1 = 128B swizzle with 32B
-//                                                atoms, 2 = 128B swizzle, 4 = 64B, 6 = 32B
-// Tile bases are 1024-byte aligned; tiles are written by TMA with the matching swizzle.
-//   K-major operand  (CU_TENSOR_MAP_SWIZZLE_128B, layout 2): rows of 128 B (one swizzle
-//       row) along K, 8-row atoms 1024 B apart along M/N -> SBO = 1024, LBO unused.
-//   MN-major 16-bit  (CU_TENSOR_MAP_SWIZZLE_128B, layout 2): 128 B along M/N per k row,
-//       8 k-rows = one atom (SBO = 1024 between atoms); the next 128-byte chunk of M/N is
-//       one TMA box further (LBO = box bytes).
-//   MN-major tf32    (CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, layout 1): the only MN-major
-//       layout the tensor core accepts for 32-bit operands: 32-byte chunks swizzled over
-//       4 k-rows -> atoms of 4 k-rows, SBO = 512; LBO = box bytes as above.
-constexpr uint32_t kLayoutSw128 = 2;
-constexpr uint32_t kLayoutSw128Base32 = 1;
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes, uint32_t layout) {
+// wgmma shared-memory matrix descriptor (64 bit):
+//   [0,14)  start address >> 4          [16,30) leading-dimension byte offset >> 4
+//   [32,46) stride-dimension byte offset >> 4    [49,52) base offset = 0
+//   [62,64) layout: 0 none, 1 = 128B swizzle, 2 = 64B, 3 = 32B
+// Tile bases are 1024-byte aligned; tiles are written by TMA with the matching swizzle (CU_TENSOR_MAP_SWIZZLE_128B).
+//   K-major operand: rows of 128 B (one swizzle row) along K, 8-row atoms 1024 B apart along M/N -> SBO = 1024, LBO
+//       unused; the k-steps of one row advance the start address by 32 bytes.
+//   MN-major 16-bit: 128 B along M/N per k row, 8 k-rows = one atom (SBO = 1024 between atoms); the next 128-byte chunk
+//       of M/N is one TMA box further (LBO = box bytes).
+constexpr uint32_t kLayoutSw128 = 1;
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout) << 61;
+  d |= static_cast<uint64_t>(layout) << 62;
   return d;
 }
-
-// Instruction descriptor (32 bit) for kind::tf32 / kind::f16, dense, fp32 accumulate:
-//   [4,6) D format: 1 = F32     [7,10) A format, [10,13) B format: 0 F16, 1 BF16, 2 TF32
-//   [15] A major, [16] B major: 0 = K-major, 1 = MN-major
-//   [17,23) N >> 3              [24,29) M >> 4
+// operand formats of the kernel families (template tags; wgmma names the format in the instruction itself)
 constexpr uint32_t kFmtF16 = 0, kFmtBF16 = 1, kFmtTF32 = 2;
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t fmt, uint32_t a_mn_major,
-                                                  uint32_t b_mn_major, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
 
 }  // namespace ptx
 }  // namespace lb200

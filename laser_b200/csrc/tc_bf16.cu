@@ -1,4 +1,4 @@
-// tc_bf16.cu -- the eight instantiations (operand major-ness x single CTA / CTA pair) of gemm_tc_kernel<2, ptx::kFmtBF16, 1, uint16_t, false>
+// tc_bf16.cu -- the eight instantiations (operand major-ness x single CTA / cluster of two) of gemm_tc_kernel<2, ptx::kFmtBF16, 1, uint16_t, false>
 #include "tc_launch_impl.cuh"
 
 namespace lb200 {

@@ -1,4 +1,4 @@
-// tc_f16x3.cu -- the eight instantiations (operand major-ness x single CTA / CTA pair) of gemm_tc_kernel<2, ptx::kFmtF16, 3, float, true>
+// tc_f16x3.cu -- the eight instantiations (operand major-ness x single CTA / cluster of two) of gemm_tc_kernel<2, ptx::kFmtF16, 3, float, true>
 #include "tc_launch_impl.cuh"
 
 namespace lb200 {

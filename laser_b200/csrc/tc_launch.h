@@ -11,19 +11,18 @@ namespace lb200 {
 
 struct TcLaunch {
   CUtensorMap a0, a1, b0, b1;   // piece 0 (hi / the operand itself) and piece 1 (lo) of A and B
-  CUtensorMap c;                // C as a tensor of 32 x 32 boxes (used when p.c_tma; zero-initialised otherwise)
   TcParams p;
   bool a_mn = false, b_mn = false;   // operand major-ness
-  bool pair = false;                 // clusters of two CTAs (cta_group::2)
+  bool pair = false;                 // clusters of two CTAs sharing one tile scheduler
   bool pdl = false;                  // programmatic dependent launch: overlap the prologue with the preceding kernel's tail
   int dev = 0, sm_count = 0;
   cudaStream_t stream = nullptr;
 };
 
 // each returns a cudaError_t value (0 = launched)
-int launch_tc_tf32x1(const TcLaunch &l);   // fp32 in/out, kind::tf32, one pass (hardware truncates fp32 -> tf32)
-int launch_tc_tf32x3(const TcLaunch &l);   // fp32 in/out, kind::tf32, hi/lo pieces, three passes
-int launch_tc_bf16(const TcLaunch &l);     // bf16 in/out, kind::f16
+int launch_tc_tf32x1(const TcLaunch &l);   // fp32 in/out, wgmma tf32, one pass (the tensor core ignores the low mantissa bits)
+int launch_tc_tf32x3(const TcLaunch &l);   // fp32 in/out, wgmma tf32, hi/lo pieces, three passes
+int launch_tc_bf16(const TcLaunch &l);     // bf16 in/out, wgmma bf16
 int launch_tc_f16x3(const TcLaunch &l);    // two fp16 pieces of the scaled fp32 operands, three passes, fp32 out (default fp32 mode)
 
 }  // namespace lb200

@@ -17,7 +17,7 @@ template <int ESZ, uint32_t FMT16, int NPASS, typename OutT, bool SCALED, bool P
 int launch_tc_one(const TcLaunch &l) {
   using Cfg = TcCfg<NPASS, PAIR>;
   const int64_t units_total = tc_units(l.p);  // work units
-  // persistent: one CTA (or one CTA pair) per SM (pair of SMs), never more CTAs than units
+  // persistent: one CTA (or one cluster of two) per SM (pair of SMs), never more CTAs than units
   const int units = PAIR ? l.sm_count / 2 : l.sm_count;
   const int sched = static_cast<int>(units_total < units ? units_total : units);
   cudaLaunchConfig_t cfg{};
@@ -44,11 +44,16 @@ int launch_tc_one(const TcLaunch &l) {
     if (e != cudaSuccess) return static_cast<int>(e);
     attr_set.fetch_or(1u << l.dev, std::memory_order_release);
   }
-  return static_cast<int>(LB200_LAUNCH_EX(&cfg, kfn, l.a0, l.a1, l.b0, l.b1, l.c, l.p));
+  return static_cast<int>(LB200_LAUNCH_EX(&cfg, kfn, l.a0, l.a1, l.b0, l.b1, l.p));
 }
 
 template <int ESZ, uint32_t FMT16, int NPASS, typename OutT, bool SCALED>
 int launch_tc_family(const TcLaunch &l) {
+  if constexpr (ESZ == 4) {   // wgmma reads tf32 tiles K-major only: capi.cu prepares MN-major fp32 operands K-major
+    if (l.a_mn || l.b_mn) return static_cast<int>(cudaErrorNotSupported);
+    if (l.pair) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, true, false, false>(l);
+    return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, false, false, false>(l);
+  }
 #define LB200_MAJORS(PAIR)                                                                                   \
   do {                                                                                                       \
     if (!l.a_mn && !l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, false, false>(l);    \
@@ -56,8 +61,10 @@ int launch_tc_family(const TcLaunch &l) {
     if (l.a_mn && !l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, true, false>(l);      \
     return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, true, true>(l);                              \
   } while (0)
-  if (l.pair) LB200_MAJORS(true);
-  LB200_MAJORS(false);
+  if constexpr (ESZ == 2) {
+    if (l.pair) LB200_MAJORS(true);
+    LB200_MAJORS(false);
+  }
 #undef LB200_MAJORS
 }
 

@@ -13,35 +13,29 @@
 namespace lb200 {
 
 constexpr int TC_BLOCK_M = 128;
-constexpr int TC_BLOCK_N = 256;
+constexpr int TC_BLOCK_N = 128;
 constexpr int TC_ROW_BYTES = 128;  // one swizzle row; BLOCK_K = 128 / sizeof(element)
 constexpr int TC_A_TILE_BYTES = TC_BLOCK_M * TC_ROW_BYTES;  // 16 KB: 128 rows x 128 B
 template <int NPASS, bool PAIR> struct TcCfg {
   static constexpr int PIECES = (NPASS == 3) ? 2 : 1;
-  static constexpr int B_COLS = PAIR ? TC_BLOCK_N / 2 : TC_BLOCK_N;
-  static constexpr int B_TILE_BYTES = B_COLS * TC_ROW_BYTES;
+  static constexpr int B_TILE_BYTES = TC_BLOCK_N * TC_ROW_BYTES;
   static constexpr int A_STAGE_BYTES = PIECES * TC_A_TILE_BYTES;
   static constexpr int B_STAGE_BYTES = PIECES * B_TILE_BYTES;
-  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;  // 32 / 48 KB (1 pass), 64 / 96 KB (3 passes)
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;  // 32 KB (1 pass), 64 KB (3 passes)
 #ifdef TC_STAGES_OVERRIDE
   static constexpr int STAGES = TC_STAGES_OVERRIDE;
 #else
-  static constexpr int STAGES = (NPASS == 3) ? (PAIR ? 3 : 2) : (PAIR ? 6 : 4);   // 192 KB of tiles in every variant
+  static constexpr int STAGES = (NPASS == 3) ? 3 : 6;   // 192 KB of tiles in every variant (227 KB per block on sm_90)
 #endif
-  // after the operand stages: one 4 KB staging buffer per epilogue warp (32 rows x 128 B, 128B-swizzled) from which the
-  // tile leaves through cp.async.bulk.tensor stores, then the barriers
-  static constexpr int STORE_STAGING_BYTES = 8 * 32 * 128;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STORE_STAGING_BYTES + 1024 /*align*/ + 512 /*barriers, scheduler slot*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 512 /*barriers, scheduler slot*/;
 };
-constexpr int TC_ACC_STAGES = 2;
-constexpr int TC_TMEM_COLS = TC_ACC_STAGES * TC_BLOCK_N;  // 512: all of TMEM
-// warp 0 TMA, 1 MMA, 2 TMEM alloc, 3 tile scheduler | warps 4-11: epilogue (2 warpgroups)
+// warpgroup 0: warp 0 TMA, warp 3 tile scheduler | warpgroups 1, 2: wgmma + epilogue, 64 rows each
 constexpr int TC_THREADS = 384;
 constexpr int TC_EPI_THREADS = 256;
 constexpr int TC_EPI_WARPS = TC_EPI_THREADS / 32;
-constexpr int TC_EPI_COLS = TC_BLOCK_N / 2;  // columns owned by one epilogue thread
-constexpr int TC_REGS_CTRL = 56;   // setmaxnreg for the producer/MMA warpgroup
-constexpr int TC_REGS_EPI = 224;   // ... and for the epilogue warpgroups (running sums): 4 x 32 x 56 + 8 x 32 x 224 = the 64512 of the launch
+constexpr int TC_ACC_REGS = 64 * TC_BLOCK_N / 128;   // fp32 accumulators per thread of an m64 x n128 wgmma
+constexpr int TC_REGS_CTRL = 40;   // setmaxnreg for the producer / scheduler warpgroup
+constexpr int TC_REGS_EPI = 232;   // ... and for the consumer warpgroups (accumulators + running sums): 128 x 40 + 256 x 232 <= 65536
 
 // fused epilogue: v -> act(v + bias)   (gemm.nim:196 "elementwise epilogue fusion")
 struct Epilogue {
@@ -54,7 +48,7 @@ struct TcParams {
   float alpha, beta;
   void *C;
   int64_t rsC, csC;
-  int kb_per_block;   // k-tiles per TMEM accumulation block (>= 1)
+  int kb_per_block;   // k-tiles per accumulation block of the wgmma registers (>= 1)
   uint32_t zero;      // always 0; opaque to the compiler (see the epilogue)
   int raster_g;       // m-blocks per raster group (see tile_coords)
   Epilogue epi;
@@ -64,15 +58,12 @@ struct TcParams {
   // alpha / beta / bias / activation) to the tile-local plane [s][i] of split_ws; splitk_tail_reduce_kernel then adds the
   // planes in order and applies alpha / beta / epilogue.  Two uses: few output tiles and a long K (n_direct = 0: every
   // tile is split), and the partial last wave of a persistent launch (n_direct = the tiles of the full waves: the
-  // remainder of 4096^3's 256 pair-tiles on 74 SM pairs runs as 68 half-K units instead of 34 full ones: 3.5 waves, not 4)
+  // remainder of at most half a wave runs as twice as many half-K units, which the idle SMs take up)
   int n_direct;          // == num_m_blocks * num_n_blocks when nothing is split
   int k_splits;          // >= 1
   int kb_per_split;      // k-tiles per split
   float *split_ws = nullptr;   // [k_splits][split tiles][tile rows][TC_BLOCK_N] fp32
-  int num_m_blocks, num_n_blocks;  // output tiles: 128 x 256, or 256 x 256 per CTA pair
-  // fp32 C with unit column stride and 16-byte aligned rows leaves through TMA (mapC of the launch: box 32 columns x 32 rows,
-  // 128B swizzle; rows / columns past M / N are clipped by the copy engine); otherwise, and for split units, plain stores
-  int c_tma = 0;
+  int num_m_blocks, num_n_blocks;  // output tiles: 128 x 128, or 256 x 128 per cluster of two CTAs
   // SCALED: fp32 bits of the largest finite |a| of row i of A / |b| of column j of B (f16_scale.cuh)
   const uint32_t *amax_a = nullptr, *amax_b = nullptr;
   // tile scheduler: word 0 = next unit (atomicAdd), word 1 = pairs that have drawn their last unit (the last one zeroes
@@ -80,9 +71,9 @@ struct TcParams {
   unsigned int *sched = nullptr;
 };
 
-// raster order of the output tiles: groups of G m-blocks sweep n together, so that the concurrently resident tiles (148 of
-// 128 x 256, or 74 pairs of 256 x 256) cover a near-square patch, which minimises the A + B panels one wave pulls through
-// L2 (G = 16 single-CTA tiles / 8 pair tiles = 2048 rows)
+// raster order of the output tiles: groups of G m-blocks sweep n together, so that the concurrently resident tiles (132 of
+// 128 x 128 on an H100 SXM, or 66 cluster tiles of 256 x 128) cover a compact patch, which limits the A + B panels one wave
+// pulls through L2 (G = 16 single-CTA tiles / 8 cluster tiles = 2048 rows)
 LB200_HD inline void tile_coords(int t, int num_m, int num_n, int G, int &mb, int &nb) {
   const int per_group = G * num_n;
   const int g = t / per_group;
@@ -96,7 +87,7 @@ LB200_HD inline void tile_coords(int t, int num_m, int num_n, int G, int &mb, in
 // host side: the part of TcParams that depends only on the problem (p.M, p.N, p.K set by the
 // caller) and on the configuration
 struct TcPlanCfg {
-  int kc_faithful;      // K extent per TMEM accumulation block in the fp32-faithful modes
+  int kc_faithful;      // K extent per accumulator block in the fp32-faithful modes
   int raster_g;         // 0 = default
   bool splitk_enabled;
   int sm_count;

@@ -1,4 +1,4 @@
-"""Backend of the `-m gpu` test files: a B200 through torch CUDA tensors, or -- LASER_B200_EMU=1, set by
+"""Backend of the `-m gpu` test files: an H100 through torch CUDA tensors, or -- LASER_B200_EMU=1, set by
 tests/test_emulated_python_mirror.py together with LASER_B200_LIB -- the host-emulated build of the
 library, where "device" memory is host memory held by numpy arrays."""
 import os

@@ -1,6 +1,6 @@
 // conv_selftests.cpp -- the reference's convolution self-check (`conv_impl_check`,
 // benchmarks/convolution/conv2d_common.nim:128-283) and a transposition check (swapaxes.nim:16-112)
-// re-stated against the C++ host mirror (include/laser_b200.hpp).  Needs a B200 to run; with
+// re-stated against the C++ host mirror (include/laser_b200.hpp).  Needs an H100 to run; with
 // --link-only it only proves that the mirror compiles and links.
 #include <cstdio>
 #include <cstring>

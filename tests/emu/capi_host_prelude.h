@@ -26,7 +26,7 @@ template <typename... KArgs, typename... Args>
 inline void launch_kernel(void (*kernel)(KArgs...), unsigned grid, unsigned block, cudaStream_t s, Args &&...args) {
   emu_launch_kernel(kernel, grid, block, 0, s, static_cast<Args &&>(args)...);
 }
-// cudaLaunchKernelEx with a cluster dimension (the tcgen05 kernel)
+// cudaLaunchKernelEx with a cluster dimension (the wgmma kernel)
 template <typename... KArgs, typename... Args>
 inline cudaError_t emu_launch_ex(const cudaLaunchConfig_t *cfg, void (*kernel)(KArgs...), Args &&...args) {
   unsigned cluster = 1;
@@ -88,7 +88,7 @@ cudaError_t cudaSetDevice(int d) {
 cudaError_t cudaGetDeviceCount(int *n) { *n = emu_device_count(); return cudaSuccess; }
 cudaError_t cudaGetDeviceProperties_v2(cudaDeviceProp *p, int) {
   std::memset(p, 0, sizeof *p);
-  p->major = 10; p->minor = 0; p->multiProcessorCount = emu_device_count_sms();
+  p->major = 9; p->minor = 0; p->multiProcessorCount = emu_device_count_sms();
   return cudaSuccess;
 }
 cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, unsigned) { static long n = 0x100; *s = reinterpret_cast<cudaStream_t>(n += 0x10); return cudaSuccess; }

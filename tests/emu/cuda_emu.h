@@ -4,7 +4,7 @@
 // pthread barrier for __syncthreads, clusters of CTAs running side by side, clusters one after the
 // other.  Kernels written in plain CUDA C++ run as they are (layers.cuh, gemm_simt.cuh, split.cuh
 // with a software tf32 rounding; of the warp intrinsics only full-mask __shfl_xor_sync and
-// __syncwarp are modelled); the tcgen05 kernel runs on top of ptx_emu.h, a functional model of
+// __syncwarp are modelled); the wgmma kernel runs on top of ptx_emu.h, a functional model of
 // the PTX it uses.  It is a test of the product's source, not a fallback: nothing under laser_b200/
 // can reach it.
 #pragma once
@@ -38,7 +38,7 @@
 
 namespace emu {
 constexpr unsigned kMaxCluster = 2;                 // CTAs running side by side
-constexpr size_t kDynSmemBytes = 232448;            // 227 KB, the sm_100 limit per CTA
+constexpr size_t kDynSmemBytes = 232448;            // 227 KB, the sm_90 limit per CTA
 struct Idx {
   unsigned x, y, z;
 };

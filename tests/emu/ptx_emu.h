@@ -1,20 +1,22 @@
 // ptx_emu.h -- TEST INFRASTRUCTURE: a functional model of the PTX that laser_b200/csrc/ptx.cuh
-// wraps (mbarrier, cp.async.bulk.tensor, tcgen05.alloc/mma/commit/ld, clusters of two CTAs), under
-// the same names, so that gemm_tc.cuh -- the tcgen05 kernel -- can be compiled by g++ and run on host
-// threads (cuda_emu.h).  What the model checks: the producer / MMA / epilogue protocol (barrier
-// counts, phases, stage rings: a protocol error shows up as a deadlock or as a wrong sum), the tile
-// scheduler, raster and split-K ranges, the k-block bookkeeping of every mode, operand addressing
-// through the descriptors' start / LBO / SBO fields, out-of-bounds zero fill, the CTA-pair
-// ownership of rows and columns, and every epilogue path.  What it cannot check: anything that is
-// a property of the silicon -- the 128-byte swizzle patterns (tiles are kept unswizzled here, on
-// both the TMA and the MMA side), instruction encodings, memory-proxy fences, register limits,
-// the accumulator's rounding (modelled: tf32 operands truncated, exact products, one rounding per
-// instruction).  Those are covered by the -m gpu tests only.
+// wraps (mbarrier, cp.async.bulk.tensor, wgmma, clusters of two CTAs), under the same names, so
+// that gemm_tc.cuh -- the wgmma kernel -- can be compiled by g++ and run on host threads
+// (cuda_emu.h).  What the model checks: the producer / consumer protocol (barrier counts, phases,
+// stage rings: a protocol error shows up as a deadlock or as a wrong sum), the tile scheduler,
+// raster and split-K ranges, the k-block bookkeeping of every mode, operand addressing through the
+// descriptors' start / LBO / SBO fields, the accumulator fragment layout the epilogue assumes,
+// out-of-bounds zero fill, the cluster's ownership of rows, and every epilogue path.  What it
+// cannot check: anything that is a property of the silicon -- the 128-byte swizzle patterns (tiles
+// are kept unswizzled here, on both the TMA and the MMA side), instruction encodings, the
+// asynchrony of wgmma (an instruction completes when it is issued here), memory-proxy fences,
+// register limits, the accumulator's rounding (modelled: tf32 operands truncated, exact products,
+// one rounding per instruction).  Those are covered by the -m gpu tests only.
 #pragma once
 
 #include <cuda.h>
 #include <stdint.h>
 
+#include <chrono>
 #include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
@@ -48,7 +50,6 @@ struct MBarrier {
 inline std::mutex mb_mu;
 inline std::condition_variable mb_cv;
 inline std::map<const void *, MBarrier> mbars;
-inline float tmem[kMaxCluster][128][512];   // TMEM of each CTA: 128 lanes x 512 columns of 32 bits
 
 inline void reset_state() {
   std::lock_guard<std::mutex> lk(mb_mu);
@@ -120,10 +121,31 @@ inline bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
   std::lock_guard<std::mutex> lk(emu::mb_mu);
   return emu::mb_get(bar).phase != parity;
 }
+// seconds one thread may wait on one mbarrier before the wait is reported as a deadlock: env LASER_B200_EMU_WAIT_S
+// (default 120), ten times that in a sanitizer build, where everything runs several times slower
+inline int mbar_wait_limit_s() {
+  static const int limit = []() {
+    const char *e = std::getenv("LASER_B200_EMU_WAIT_S");
+    int v = e ? std::atoi(e) : 0;
+    if (v <= 0) v = 120;
+#if defined(__SANITIZE_ADDRESS__) || defined(__SANITIZE_THREAD__)
+    v *= 10;
+#endif
+    return v;
+  }();
+  return limit;
+}
 inline void mbar_wait(uint64_t *bar, uint32_t parity) {   // blocking (hundreds of waiters on a few cores)
   std::unique_lock<std::mutex> lk(emu::mb_mu);
   emu::MBarrier &b = emu::mb_get(bar);
-  emu::mb_cv.wait(lk, [&]() { return b.phase != parity; });
+  // a protocol error is a deadlock: past the limit, report the barrier and the waiting thread instead of hanging
+  if (!emu::mb_cv.wait_for(lk, std::chrono::seconds(mbar_wait_limit_s()), [&]() { return b.phase != parity; })) {
+    std::fprintf(stderr, "emu: deadlock: thread %u of CTA rank %u waits for parity %u of the mbarrier at shared offset %u "
+                 "(pending %d of %d arrivals, tx %ld)\n", emu::t_idx.x, emu::cta_rank, parity,
+                 static_cast<unsigned>(smem_u32(bar) & 0xFFFFFF), b.pending, b.init_count, b.tx);
+    emu::mb_cv.wait_for(lk, std::chrono::seconds(5));   // the other blocked threads report too
+    std::abort();
+  }
 }
 
 // ----------------------------------------------------------------------- TMA
@@ -167,30 +189,6 @@ inline void cp_async_16(void *smem_dst, const void *gsrc, uint32_t src_bytes) {
 }
 inline void cp_async_commit() {}
 template <int N> inline void cp_async_wait() {}
-inline int sw128_chunk(int, int j) { return j; }      // the model keeps tiles unswizzled on both sides
-// cp.async.bulk.tensor store: the box leaves at once (commit / wait have nothing to track); elements outside the tensor are
-// not written
-inline void tma_store_2d(const CUtensorMap *map, const void *smem_src, int32_t c0, int32_t c1) {
-  emu::TensorMap2D m;
-  std::memcpy(&m, map, sizeof m);
-  if (m.magic != emu::kMapMagic) { std::fprintf(stderr, "emu: not an emulated tensor map\n"); std::abort(); }
-  const unsigned char *src = static_cast<const unsigned char *>(smem_src);
-  const unsigned char *lo = emu::dyn_smem[emu::cta_rank];
-  const size_t box_bytes = static_cast<size_t>(m.box0) * m.box1 * m.esz;
-  if (src < lo || src + box_bytes > lo + emu::kDynSmemBytes || ((src - lo) & 1023)) {
-    std::fprintf(stderr, "emu: TMA store source outside this CTA's shared memory or not 1024-byte aligned\n");
-    std::abort();
-  }
-  for (int r = 0; r < m.box1; ++r)
-    for (int e = 0; e < m.box0; ++e) {
-      const int64_t i0 = static_cast<int64_t>(c0) + e, i1 = static_cast<int64_t>(c1) + r;
-      if (i0 >= 0 && i0 < m.dim0 && i1 >= 0 && i1 < m.dim1)
-        std::memcpy(const_cast<unsigned char *>(m.base) + i1 * m.stride1_bytes + i0 * m.esz, src + (static_cast<size_t>(r) * m.box0 + e) * m.esz, m.esz);
-    }
-}
-inline void tma_store_commit() {}
-template <int N> inline void tma_store_wait_read() {}
-template <int N> inline void tma_store_wait() {}
 inline void bulk_load_1d(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar) {
   if ((reinterpret_cast<uintptr_t>(smem_dst) | reinterpret_cast<uintptr_t>(gsrc) | bytes) & 15u) std::abort();   // the hardware faults
   std::memcpy(smem_dst, gsrc, bytes);
@@ -213,51 +211,47 @@ inline void tma_load_2d_hint(void *smem_dst, const CUtensorMap *map, uint64_t *b
   tma_load_2d(smem_dst, map, bar, c0, c1);   // cache policies have no functional effect
 }
 
-// ------------------------------------------------------------------- tcgen05
-inline void tc_fence_before_sync() {}
-inline void tc_fence_after_sync() {}
-template <uint32_t NCOLS> inline void tmem_alloc(uint32_t *smem_dst) { *smem_dst = 0; }   // whole warp, same value
-template <uint32_t NCOLS> inline void tmem_dealloc(uint32_t) {}
+// ------------------------------------------------------------------- wgmma
+inline void wgmma_fence() {}
+inline void wgmma_commit() {}
+// .sync.aligned: every lane of the warp has issued (and, in this model, completed) its MMAs before any lane goes on -- lane 0
+// then releases the stage for the whole warp
+template <int N> inline void wgmma_wait() { pthread_barrier_wait(&emu::warp_barrier[emu::cta_rank][emu::t_idx.x >> 5]); }
+inline void wgmma_hold(float (&)[64]) {}
 
-constexpr uint32_t kLayoutSw128 = 2;
-constexpr uint32_t kLayoutSw128Base32 = 1;
+constexpr uint32_t kLayoutSw128 = 1;
 inline uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout) << 61;
+  d |= static_cast<uint64_t>(layout) << 62;
   return d;
 }
 constexpr uint32_t kFmtF16 = 0, kFmtBF16 = 1, kFmtTF32 = 2;
-constexpr uint32_t make_idesc(uint32_t fmt, uint32_t a_mn_major, uint32_t b_mn_major, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
 
 // one operand element as fp32: tile kept UNSWIZZLED in shared memory, addressed through the
 // descriptor fields the way the canonical layouts define them:
 //   K-major : row i at (i / 8) * SBO + (i % 8) * 128, k inside the 128-byte row
-//   MN-major: 128-byte chunk c of the mn extent at c * LBO, k-row kk at (kk / R) * SBO + (kk % R) * 128,
-//             R = 4 k-rows per atom for the 32-byte-atom layout, 8 otherwise
+//   MN-major: 128-byte chunk c of the mn extent at c * LBO, k-row kk at (kk / 8) * SBO + (kk % 8) * 128
 inline float operand_elem(const unsigned char *cta_smem, uint64_t desc, bool mn_major, int E, uint32_t fmt, int i, int kk) {
   const uint32_t start = static_cast<uint32_t>(desc & 0x3FFF) << 4;
   const uint32_t lbo = static_cast<uint32_t>((desc >> 16) & 0x3FFF) << 4;
   const uint32_t sbo = static_cast<uint32_t>((desc >> 32) & 0x3FFF) << 4;
-  const uint32_t layout = static_cast<uint32_t>(desc >> 61);
+  if (static_cast<uint32_t>(desc >> 62) != kLayoutSw128) { std::fprintf(stderr, "emu: descriptor without the 128B swizzle\n"); std::abort(); }
   size_t off;
   if (!mn_major) {
     off = start + static_cast<size_t>(i / 8) * sbo + static_cast<size_t>(i % 8) * 128 + static_cast<size_t>(kk) * E;
   } else {
-    const int per_chunk = 128 / E, R = (layout == kLayoutSw128Base32) ? 4 : 8;
-    off = start + static_cast<size_t>(i / per_chunk) * lbo + static_cast<size_t>(kk / R) * sbo +
-          static_cast<size_t>(kk % R) * 128 + static_cast<size_t>(i % per_chunk) * E;
+    const int per_chunk = 128 / E;
+    off = start + static_cast<size_t>(i / per_chunk) * lbo + static_cast<size_t>(kk / 8) * sbo +
+          static_cast<size_t>(kk % 8) * 128 + static_cast<size_t>(i % per_chunk) * E;
   }
   if (off + E > emu::kDynSmemBytes) { std::fprintf(stderr, "emu: operand read outside shared memory\n"); std::abort(); }
   if (E == 4) {
     uint32_t u;
     std::memcpy(&u, cta_smem + off, 4);
-    if (fmt == kFmtTF32) u &= 0xffffe000u;   // kind::tf32 ignores the low 13 mantissa bits
+    if (fmt == kFmtTF32) u &= 0xffffe000u;   // tf32 ignores the low 13 mantissa bits
     return __uint_as_float(u);
   }
   uint16_t h;
@@ -274,61 +268,36 @@ inline float operand_elem(const unsigned char *cta_smem, uint64_t desc, bool mn_
   return __uint_as_float(static_cast<uint32_t>(h) << 16);
 }
 
-// D[tmem] (+)= A * B for one instruction (K = 32 bytes per operand row).  ncta = 1: M x N from this
-// CTA's shared memory into this CTA's TMEM.  ncta = 2: rows [0,128) of A and of D belong to CTA 0,
-// rows [128,256) to CTA 1; columns [0,N/2) of B come from CTA 0, [N/2,N) from CTA 1.
-inline void mma_model(int ncta, int E, uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  const uint32_t fmt = (idesc >> 7) & 7;
-  const bool a_mn = (idesc >> 15) & 1, b_mn = (idesc >> 16) & 1;
-  const int N = static_cast<int>((idesc >> 17) & 63) << 3, M = static_cast<int>((idesc >> 24) & 31) << 4;
+// D (64 x 128) (+)= A (64 x K) * B (K x 128) for one instruction (K = 32 bytes per operand row), operands from THIS CTA's
+// shared memory.  Every thread of the warpgroup computes its own fragment: thread t holds rows 16 (t / 32) + (t % 32) / 4
+// (+ 8) and columns 8 i + 2 (t % 4) + {0, 1}, d[4 i + 2 h + e] (ptx.cuh).
+inline void wgmma_model(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d, int E, uint32_t fmt, bool a_mn, bool b_mn) {
+  if (E == 4 && (a_mn || b_mn)) { std::fprintf(stderr, "emu: tf32 operands must be K-major\n"); std::abort(); }
+  const unsigned t = emu::t_idx.x & 127u, w = t >> 5, lane = t & 31u;
+  const unsigned char *sm = emu::dyn_smem[emu::cta_rank];
   const int KI = 32 / E;
-  if (M != 128 * ncta || N > 256 || N % 16) { std::fprintf(stderr, "emu: unsupported MMA shape %d x %d\n", M, N); std::abort(); }
-  const uint32_t col0 = d_tmem & 0xFFFF, lane0 = d_tmem >> 16;
-  if (lane0 != 0 || col0 + N > 512) { std::fprintf(stderr, "emu: accumulator outside TMEM\n"); std::abort(); }
-  const unsigned self = emu::cta_rank;
-  static thread_local float a[256][16], b[256][16];
-  for (int i = 0; i < M; ++i) {
-    const unsigned char *sm = emu::dyn_smem[ncta == 2 ? i / 128 : self];
-    for (int kk = 0; kk < KI; ++kk) a[i][kk] = operand_elem(sm, a_desc, a_mn, E, fmt, i % 128, kk);
-  }
-  for (int j = 0; j < N; ++j) {
-    const unsigned char *sm = emu::dyn_smem[ncta == 2 ? j / (N / 2) : self];
-    const int jj = ncta == 2 ? j % (N / 2) : j;
-    for (int kk = 0; kk < KI; ++kk) b[j][kk] = operand_elem(sm, b_desc, b_mn, E, fmt, jj, kk);
-  }
-  for (int i = 0; i < M; ++i) {
-    float *drow = emu::tmem[ncta == 2 ? i / 128 : self][i % 128] + col0;
-    for (int j = 0; j < N; ++j) {
-      double s = accumulate ? static_cast<double>(drow[j]) : 0.0;
-      for (int kk = 0; kk < KI; ++kk) s += static_cast<double>(a[i][kk]) * static_cast<double>(b[j][kk]);
-      drow[j] = static_cast<float>(s);
-    }
-  }
+  float a[2][16], b[32][16];
+  for (int h = 0; h < 2; ++h)
+    for (int kk = 0; kk < KI; ++kk) a[h][kk] = operand_elem(sm, a_desc, a_mn, E, fmt, static_cast<int>(16 * w + lane / 4 + 8 * h), kk);
+  for (int i = 0; i < 16; ++i)
+    for (int e = 0; e < 2; ++e)
+      for (int kk = 0; kk < KI; ++kk) b[2 * i + e][kk] = operand_elem(sm, b_desc, b_mn, E, fmt, static_cast<int>(8 * i + 2 * (lane & 3) + e), kk);
+  for (int i = 0; i < 16; ++i)
+    for (int h = 0; h < 2; ++h)
+      for (int e = 0; e < 2; ++e) {
+        float &out = d[4 * i + 2 * h + e];
+        double s = scale_d ? static_cast<double>(out) : 0.0;
+        for (int kk = 0; kk < KI; ++kk) s += static_cast<double>(a[h][kk]) * static_cast<double>(b[2 * i + e][kk]);
+        out = static_cast<float>(s);
+      }
 }
-inline void mma_tf32_ss(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) { mma_model(1, 4, d, ad, bd, idesc, acc); }
-inline void mma_f16_ss(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) { mma_model(1, 2, d, ad, bd, idesc, acc); }
-// the instruction completes before the call returns, so a commit is an immediate arrival
-inline void mma_commit(uint64_t *bar) { emu::mb_arrive(bar, 0); }
+template <int TA, int TB>
+inline void wgmma_m64n128k16_f16(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t scale_d) { wgmma_model(d, ad, bd, scale_d, 2, kFmtF16, TA, TB); }
+template <int TA, int TB>
+inline void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t scale_d) { wgmma_model(d, ad, bd, scale_d, 2, kFmtBF16, TA, TB); }
+inline void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t scale_d) { wgmma_model(d, ad, bd, scale_d, 4, kFmtTF32, false, false); }
 
-inline void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  const uint32_t lane = (taddr >> 16) + (emu::t_idx.x & 31), col = taddr & 0xFFFF;
-  if (lane >= 128 || col + 16 > 512) { std::fprintf(stderr, "emu: tcgen05.ld outside TMEM\n"); std::abort(); }
-  if ((taddr >> 16) / 32 != ((emu::t_idx.x >> 5) & 3)) {   // a warp may only touch its own lane quarter
-    std::fprintf(stderr, "emu: warp %u reads TMEM lanes of quarter %u\n", emu::t_idx.x >> 5, (taddr >> 16) / 32);
-    std::abort();
-  }
-  for (int j = 0; j < 16; ++j) r[j] = __float_as_uint(emu::tmem[emu::cta_rank][lane][col + j]);
-}
-inline void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  uint32_t lo[16], hi[16];
-  tmem_ld_32x32b_x16(taddr, lo);
-  tmem_ld_32x32b_x16(taddr + 16, hi);
-  for (int j = 0; j < 16; ++j) { r[j] = lo[j]; r[16 + j] = hi[j]; }
-}
-inline void tmem_ld_wait(uint32_t (&)[16]) {}
-inline void tmem_ld_wait(uint32_t (&)[32]) {}
-
-// ------------------------------------------------------------ CTA pairs (cta_group::2)
+// ------------------------------------------------------------ clusters of two CTAs
 constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
 inline uint32_t cluster_ctarank() { return emu::cta_rank; }
 inline void cluster_sync() { pthread_barrier_wait(&emu::cluster_barrier); }
@@ -341,27 +310,6 @@ inline void mbar_wait_cluster(uint64_t *bar, uint32_t parity) { mbar_wait(bar, p
 inline void st_shared_cluster_s32(int *p, uint32_t rank, int v) { *reinterpret_cast<volatile int *>(emu::peer_ptr(p, rank)) = v; }
 inline void griddep_wait() {}
 inline void griddep_launch_dependents() {}
-inline void tma_load_2d_pair(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int32_t c0, int32_t c1) {
-  long bytes;
-  tma_copy_box(smem_dst, map, c0, c1, &bytes);               // into THIS CTA's shared memory
-  emu::mb_complete_tx(emu::peer_ptr(bar, 0), bytes);        // bytes credited to the LEADER's barrier
-}
-inline void tma_load_2d_pair_hint(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int32_t c0, int32_t c1, uint64_t) {
-  tma_load_2d_pair(smem_dst, map, bar, c0, c1);
-}
-inline void tma_load_3d_pair(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int32_t c0, int32_t c1, int32_t c2) {
-  long bytes;
-  tma_copy_box(smem_dst, map, c0, c1, &bytes, c2);
-  emu::mb_complete_tx(emu::peer_ptr(bar, 0), bytes);
-}
-template <uint32_t NCOLS> inline void tmem_alloc_pair(uint32_t *smem_dst) { *smem_dst = 0; }
-template <uint32_t NCOLS> inline void tmem_dealloc_pair(uint32_t) {}
-inline void mma_tf32_ss_pair(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) { mma_model(2, 4, d, ad, bd, idesc, acc); }
-inline void mma_f16_ss_pair(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) { mma_model(2, 2, d, ad, bd, idesc, acc); }
-inline void mma_commit_pair(uint64_t *bar) {   // one arrival on the barrier at this offset in BOTH CTAs
-  emu::mb_arrive(emu::peer_ptr(bar, 0), 0);
-  emu::mb_arrive(emu::peer_ptr(bar, 1), 0);
-}
 
 }  // namespace ptx
 // mma.sync.aligned.m8n8k4.row.col.f64 (gemm_dmma.cuh): lane l holds A[l / 4][l % 4], B[l % 4][l / 4] and the two accumulators

@@ -1,10 +1,12 @@
-// tc_emu.cpp -- TEST INFRASTRUCTURE: the tcgen05 GEMM kernel (laser_b200/csrc/gemm_tc.cuh) compiled
-// by g++ on top of ptx_emu.h (a functional model of mbarrier / TMA / tcgen05 / TMEM / CTA pairs) and
+// tc_emu.cpp -- TEST INFRASTRUCTURE: the wgmma GEMM kernel (laser_b200/csrc/gemm_tc.cuh) compiled
+// by g++ on top of ptx_emu.h (a functional model of mbarrier / TMA / wgmma / clusters of two CTAs) and
 // launched on host threads with the library's own planning (tc_plan) and the tensor-map parameters
 // capi.cu passes to cuTensorMapEncodeTiled (operand_map).  See ptx_emu.h for what this can and
 // cannot prove.
 #define LB200_HOST_EMULATION 1
 #include "cuda_emu.h"
+
+#include <vector>
 
 #include "../../laser_b200/csrc/gemm_tc.cuh"
 #include "../../laser_b200/csrc/split.cuh"
@@ -47,7 +49,6 @@ struct Args {
   int *out_k_splits, *out_grid;
   const uint32_t *amax_a, *amax_b;   // SCALED: abs-max words per row of A / column of B (f16_scale.cuh)
   int tail_min_k;            // TcPlanCfg::tail_min_k (0: the library's default)
-  int c_tma;                 // 1: C through TMA stores when addressable (the library's default), 0: plain stores
   int dyn_sched;             // 1: tiles drawn from an atomic counter (capi.cu: Ctx::sched), 0: static round-robin
 };
 
@@ -72,17 +73,9 @@ static int run(const Args &a) {
     if (g_sched[0] != 0u || g_sched[1] != 0u) return -4;   // the previous launch must have re-armed its slot
     p.sched = g_sched;
   }
-  const int b_block = PAIR ? TC_BLOCK_N / 2 : TC_BLOCK_N;
+  const int b_block = TC_BLOCK_N;
   const CUtensorMap mA0 = operand_map(ESZ, a.A[0], A_MN, a.M, a.K, a.ldA, TC_BLOCK_M), mA1 = operand_map(ESZ, a.A[1], A_MN, a.M, a.K, a.ldA, TC_BLOCK_M);
   const CUtensorMap mB0 = operand_map(ESZ, a.B[0], B_MN, a.N, a.K, a.ldB, b_block), mB1 = operand_map(ESZ, a.B[1], B_MN, a.N, a.K, a.ldB, b_block);
-  // capi.cu: tc_run -- fp32 C with unit column stride and 16-byte aligned rows leaves through TMA stores of 32 x 32 boxes
-  CUtensorMap mC;
-  std::memset(&mC, 0, sizeof mC);
-  if (std::is_same<OutT, float>::value && a.c_tma && a.csC == 1 && a.rsC >= a.N && (a.rsC * 4) % 16 == 0 &&
-      (reinterpret_cast<uintptr_t>(a.C) & 15) == 0 && a.N >= 32) {
-    mC = make_map(4, a.C, a.N, a.M, a.rsC, 32, 32);
-    p.c_tma = 1;
-  }
   // tc_launch_impl.cuh: launch_tc_one -- persistent: one CTA (pair) per SM (pair of SMs), never more than work units
   const int64_t units_total = tc_units(p);
   const int units = PAIR ? a.sm_count / 2 : a.sm_count;
@@ -92,7 +85,7 @@ static int run(const Args &a) {
   if (TcCfg<NPASS, PAIR>::SMEM_BYTES > static_cast<int>(emu::kDynSmemBytes)) return -3;
   emu::reset_state();
   emu::launch(grid, TC_THREADS,
-              [=]() { gemm_tc_kernel<ESZ, FMT16, NPASS, A_MN, B_MN, OutT, PAIR, SCALED>(mA0, mA1, mB0, mB1, mC, p); },
+              [=]() { gemm_tc_kernel<ESZ, FMT16, NPASS, A_MN, B_MN, OutT, PAIR, SCALED>(mA0, mA1, mB0, mB1, p); },
               PAIR ? 2 : 1);
   if (p.k_splits > 1) {
     if constexpr (std::is_same<OutT, float>::value) {
@@ -113,13 +106,38 @@ static int run(const Args &a) {
   return 0;
 }
 
+// capi.cu: prepare_operand -- the tf32 modes gather an MN-major fp32 operand ([k][ld]) into compact K-major rows
+static const void *to_k_major(const void *src, int64_t mn, int64_t k, int64_t ld, int64_t ld_out, std::vector<float> &dst) {
+  if (!src) return nullptr;
+  dst.assign(static_cast<size_t>(mn * ld_out), 0.0f);
+  const float *s = static_cast<const float *>(src);
+  for (int64_t i = 0; i < mn; ++i)
+    for (int64_t kk = 0; kk < k; ++kk) dst[i * ld_out + kk] = s[kk * ld + i];
+  return dst.data();
+}
+
 template <int ESZ, uint32_t FMT16, int NPASS, typename OutT, bool SCALED>
-static int dispatch(int a_mn, int b_mn, int pair, const Args &a) {
+static int dispatch(int a_mn, int b_mn, int pair, const Args &a_in) {
 #define GO(AMN, BMN) (pair ? run<ESZ, FMT16, NPASS, OutT, SCALED, AMN, BMN, true>(a) : run<ESZ, FMT16, NPASS, OutT, SCALED, AMN, BMN, false>(a))
-  if (!a_mn && !b_mn) return GO(false, false);
-  if (!a_mn && b_mn) return GO(false, true);
-  if (a_mn && !b_mn) return GO(true, false);
-  return GO(true, true);
+  Args a = a_in;
+  if constexpr (ESZ == 4) {
+    std::vector<float> ka[2], kb[2];
+    const int64_t ld_k = (a.K + 3) / 4 * 4;
+    if (a_mn) {
+      for (int i = 0; i < 2; ++i) a.A[i] = to_k_major(a_in.A[i], a.M, a.K, a_in.ldA, ld_k, ka[i]);
+      a.ldA = ld_k;
+    }
+    if (b_mn) {
+      for (int i = 0; i < 2; ++i) a.B[i] = to_k_major(a_in.B[i], a.N, a.K, a_in.ldB, ld_k, kb[i]);
+      a.ldB = ld_k;
+    }
+    return GO(false, false);
+  } else {
+    if (!a_mn && !b_mn) return GO(false, false);
+    if (!a_mn && b_mn) return GO(false, true);
+    if (a_mn && !b_mn) return GO(true, false);
+    return GO(true, true);
+  }
 #undef GO
 }
 
@@ -128,9 +146,9 @@ extern "C" int emu_gemm_tc(int kind, int a_mn, int b_mn, int pair, int64_t M, in
                            const void *A0, const void *A1, int64_t ldA, const void *B0, const void *B1, int64_t ldB,
                            void *C, int64_t rsC, int64_t csC, int kc_faithful, int raster_g, int splitk_enabled,
                            int sm_count, const float *bias, int bias_per_row, int act, float *splitk_ws, int64_t splitk_ws_floats, int *out_k_splits,
-                           int *out_grid, const uint32_t *amax_a, const uint32_t *amax_b, int dyn_sched, int tail_min_k, int c_tma) {
+                           int *out_grid, const uint32_t *amax_a, const uint32_t *amax_b, int dyn_sched, int tail_min_k) {
   Args a{M, N, K, alpha, beta, {A0, A1}, {B0, B1}, ldA, ldB, C, rsC, csC, kc_faithful,
-         raster_g, splitk_enabled, sm_count, bias, bias_per_row, act, splitk_ws, splitk_ws_floats, out_k_splits, out_grid, amax_a, amax_b, tail_min_k, c_tma, dyn_sched};
+         raster_g, splitk_enabled, sm_count, bias, bias_per_row, act, splitk_ws, splitk_ws_floats, out_k_splits, out_grid, amax_a, amax_b, tail_min_k, dyn_sched};
   switch (kind) {
     case 0: return dispatch<4, ptx::kFmtBF16, 1, float, false>(a_mn, b_mn, pair, a);
     case 1: return dispatch<4, ptx::kFmtBF16, 3, float, false>(a_mn, b_mn, pair, a);

@@ -76,7 +76,7 @@ def test_concurrent_callers_host_logic(tmp_path):
 
 @pytest.mark.gpu
 def test_concurrent_callers_on_gpu(tmp_path):
-    """the same harness on the B200: each thread launches on its own stream (cudaStreamPerThread), so the shared workspace
+    """the same harness on the H100: each thread launches on its own stream (cudaStreamPerThread), so the shared workspace
     is handed from stream to stream by the library's events while kernels of different callers overlap"""
     exe = build(tmp_path, THREADS_SRC, "threads_harness")
     for argv in (["4", "3", "1"], ["6", "2", "4"]):     # scale 4: shapes up to 1200 x 1040 x 288 and 512 x 512 x 4096

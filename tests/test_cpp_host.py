@@ -40,8 +40,6 @@ def test_cpp_layers_mirror_compiles_and_links(tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.skipif(os.environ.get("LASER_B200_UNVALIDATED", "0") != "1",
-                    reason="layer kernels not yet validated on a B200 (set LASER_B200_UNVALIDATED=1)")
 def test_conv_selftests_in_cpp(tmp_path):
     out = subprocess.run([build(tmp_path, CONV_SRC)], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stdout + out.stderr

@@ -2,7 +2,7 @@
 complete host side: dispatch, operand classification, tensor-map construction, workspaces, the pipelined
 host-pointer entry, the pre-packed API, split-K planning -- with g++ (kernel launches rewritten
 textually, CUDA runtime and cuTensorMapEncodeTiled replaced by stand-ins, tests/emu/capi_host_prelude.h)
-on top of the host-thread execution of every kernel, the tcgen05 one included (ptx_emu.h).  The ordinary
+on top of the host-thread execution of every kernel, the wgmma one included (ptx_emu.h).  The ordinary
 Python mirror is then loaded against that build in a subprocess (LASER_B200_LIB) and driven through the
 scenarios of tests/emu_driver.py with numpy arrays as "device" memory, each checked against the oracle.
 What this cannot show is listed in tests/emu/ptx_emu.h (silicon properties) -- and timing, of course."""
@@ -43,7 +43,8 @@ def test_split_k_planning_and_reduce(emulated_lib):
 
 
 @pytest.mark.parametrize("env", [dict(LASER_B200_PANEL_ROWS=512), dict(LASER_B200_PANEL_TAPER=1),
-                                 dict(LASER_B200_PANEL_ROWS=512, LASER_B200_PANEL_TAPER=1), dict(LASER_B200_CTA_PAIR=0),
+                                 dict(LASER_B200_PANEL_ROWS=512, LASER_B200_PANEL_TAPER=1),
+                                 dict(LASER_B200_CTA_PAIR=0), dict(LASER_B200_CTA_PAIR=1),
                                  dict(LASER_B200_F32_MODE="tf32x3"), dict(LASER_B200_DYNSCHED=0),
                                  dict(LASER_B200_KC=64, LASER_B200_RASTER=2)],
                          ids=lambda e: ",".join("%s=%s" % (k.replace("LASER_B200_", ""), v) for k, v in e.items()))
@@ -64,10 +65,11 @@ def test_rowsharded_entry_points_with_a_stand_in_nccl(emulated_lib, ndev, panels
 
 def test_f16x3_mode(emulated_lib):
     """the default fp32 mode: power-of-two scaling from a device-side abs-max, two fp16 pieces, the kernel undoing the
-    scales in its epilogue; range cases included.  Here on a 32-SM machine without CTA pairs, so that the single-CTA
-    kernel and split-K take part (the CTA-pair kernel runs the same assertions in test_emulated_python_mirror.py); in
+    scales in its epilogue; range cases included.  Here on a 32-SM machine with clusters of two CTAs (not the default), so
+    that the cluster kernel and split-K take part (the default single-CTA kernel runs the same assertions in
+    test_emulated_python_mirror.py); in
     the pipelined host-pointer entry every row panel of A gets its own scale"""
-    run(emulated_lib, "f16x3", LASER_B200_EMU_SMS=32, LASER_B200_CTA_PAIR=0, LASER_B200_KC=64)
+    run(emulated_lib, "f16x3", LASER_B200_EMU_SMS=32, LASER_B200_CTA_PAIR=1, LASER_B200_KC=64)
     run(emulated_lib, "host_entry", LASER_B200_F32_MODE="f16x3")
 
 

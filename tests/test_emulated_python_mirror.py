@@ -44,7 +44,7 @@ def _run_gpu_files(files, extra, timeout):
 
 
 def test_parity_file_subset_against_the_host_emulated_library():
-    """tests/test_gpu_parity.py is backend-neutral (tests/backend.py): the same assertions the B200 has to
+    """tests/test_gpu_parity.py is backend-neutral (tests/backend.py): the same assertions the H100 has to
     meet -- known-answer vectors on every path and dtype, bit-exactness of the exact kernel, bf16, the
     host-pointer entry, dispatch, the Tensor contract -- are checked here on the CPU build.  A fast
     subset by default; LASER_B200_EMU_FULL=1 runs the whole parity, fuzz, pre-packed and fused-epilogue

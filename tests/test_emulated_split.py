@@ -157,13 +157,14 @@ def test_pack_general_bf16(emu):
                                                       (5, 2.0, 1.0, 0, 2)])
 @pytest.mark.parametrize("n_direct,tile_m", [(0, 128), (3, 256)])
 def test_splitk_tail_reduce_is_a_fixed_order_sum(emu, S, alpha, beta, per_row, act, n_direct, tile_m):
-    """tile-local planes [S][n_tail][tile_m][256] of the tiles n_direct.. (raster order, tc_params.h: tile_coords) -> C;
+    """tile-local planes [S][n_tail][tile_m][BN] (BN = TC_BLOCK_N) of the tiles n_direct.. (raster order, tc_params.h: tile_coords) -> C;
     the direct tiles of C are not touched"""
-    M, N, G = 2 * tile_m + 23, 256 + 37, 2              # 3 x 2 tiles, ragged in both directions
-    num_m, num_n = -(-M // tile_m), -(-N // 256)
+    BN = 128                                             # tc_params.h: TC_BLOCK_N
+    M, N, G = 2 * tile_m + 23, BN + 37, 2               # 3 x 2 tiles, ragged in both directions
+    num_m, num_n = -(-M // tile_m), -(-N // BN)
     n_tail = num_m * num_n - n_direct
     rng = np.random.default_rng(2)
-    ws = rng.standard_normal((S, n_tail, tile_m, 256)).astype(np.float32)
+    ws = rng.standard_normal((S, n_tail, tile_m, BN)).astype(np.float32)
     C = rng.standard_normal((N, M)).astype(np.float32)            # column-major C: rsC = 1, csC = M
     bias = rng.standard_normal(M if per_row else N).astype(np.float32) if act else None
     c0 = C.copy()
@@ -182,8 +183,8 @@ def test_splitk_tail_reduce_is_a_fixed_order_sum(emu, S, alpha, beta, per_row, a
     for ti in range(n_tail):
         mb, nb = coords(n_direct + ti)
         seen.add((mb, nb))
-        r0, c0_ = mb * tile_m, nb * 256
-        rows, cols = min(tile_m, M - r0), min(256, N - c0_)
+        r0, c0_ = mb * tile_m, nb * BN
+        rows, cols = min(tile_m, M - r0), min(BN, N - c0_)
         s = ws[0, ti, :rows, :cols].copy()
         for k in range(1, S):
             s = s + ws[k, ti, :rows, :cols]                          # planes in order 0..S-1, fp32

@@ -1,9 +1,9 @@
-"""CPU-only: the tcgen05 GEMM kernel (laser_b200/csrc/gemm_tc.cuh) executed on host threads on top of a
-functional model of the PTX it uses (tests/emu/ptx_emu.h: mbarrier, TMA boxes with zero fill, tcgen05.mma
-through the shared-memory / instruction descriptors, TMEM, CTA pairs), launched with the library's own
-planning (tc_plan).  Covered: the producer / MMA / epilogue protocol of all modes (a protocol error is a
+"""CPU-only: the wgmma GEMM kernel (laser_b200/csrc/gemm_tc.cuh) executed on host threads on top of a
+functional model of the PTX it uses (tests/emu/ptx_emu.h: mbarrier, TMA boxes with zero fill, wgmma
+through the shared-memory descriptors and its accumulator fragments, clusters of two CTAs), launched with the
+library's own planning (tc_plan).  Covered: the producer / consumer / epilogue protocol of all modes (a protocol error is a
 deadlock -> timeout, or a wrong sum), tile scheduler + raster, kc-blocked accumulation, split-K, ragged
-M / N / K, K-major and MN-major operands, single CTAs and CTA pairs, every epilogue path.  Not covered
+M / N / K, K-major and MN-major operands, single CTAs and clusters of two, every epilogue path.  Not covered
 (silicon properties, see ptx_emu.h): swizzle patterns, encodings, the accumulator's rounding."""
 import ctypes
 
@@ -26,7 +26,7 @@ def emu():
     L = ctypes.CDLL(build_emu("tc_emu", ["gemm_tc.cuh", "tc_params.h", "f16_scale.cuh", "ptx.cuh", "split.cuh"]))
     L.emu_gemm_tc.restype = ci
     L.emu_gemm_tc.argtypes = [ci, ci, ci, ci, i64, i64, i64, f32, f32, vp, vp, i64, vp, vp, i64, vp, i64, i64, ci, ci, ci, ci,
-                              vp, ci, ci, vp, i64, ctypes.POINTER(ci), ctypes.POINTER(ci), vp, vp, ci, ci, ci]
+                              vp, ci, ci, vp, i64, ctypes.POINTER(ci), ctypes.POINTER(ci), vp, vp, ci, ci]
     return L
 
 
@@ -53,7 +53,7 @@ def ptr(a):
 
 
 def run_tc(emu, mode, a, b, c, rsC, csC, alpha=1.0, beta=0.0, a_mn=False, b_mn=False, pair=False, kc=128, raster=0,
-           splitk=1, sms=4, epi=None, c_base=None, dyn=1, tail_min_k=0, c_tma=1):
+           splitk=1, sms=4, epi=None, c_base=None, dyn=1, tail_min_k=0):
     """a: logical (M, K) fp32; b: logical (K, N) fp32; c: flat output buffer (float32, or uint16 for bf16).
     Returns (expected sum A*B in float64 under the mode's operand model, k_splits, grid); run_tc.n_direct holds the number
     of tiles the last launch computed without splitting (tc_params.h)."""
@@ -98,7 +98,7 @@ def run_tc(emu, mode, a, b, c, rsC, csC, alpha=1.0, beta=0.0, a_mn=False, b_mn=F
     rc = emu.emu_gemm_tc(KIND[mode], int(a_mn), int(b_mn), int(pair), M, N, K, alpha, beta,
                          ptr(arrs["A"][0]), ptr(arrs["A"][1]), ld["A"], ptr(arrs["B"][0]), ptr(arrs["B"][1]), ld["B"],
                          ctypes.c_void_p(c.ctypes.data + (c_base or 0) * c.itemsize), rsC, csC, kc, raster, splitk, sms,
-                         ptr(bias), per_row, act, ptr(ws), ws.size, ks, ctypes.byref(grid), ptr(amax["A"]), ptr(amax["B"]), dyn, tail_min_k, c_tma)
+                         ptr(bias), per_row, act, ptr(ws), ws.size, ks, ctypes.byref(grid), ptr(amax["A"]), ptr(amax["B"]), dyn, tail_min_k)
     assert rc == 0          # (the harness runs the reduce kernel of a split launch itself, like capi.cu: tc_run)
     run_tc.n_direct = ks[1]
     return exact, ks[0], grid.value
@@ -117,7 +117,7 @@ def test_modes_majorness_and_pairs(emu, mode, dyn, a_mn, b_mn, pair):
     a, b = rnd((M, K), 1), rnd((K, N), 2)
     c = np.full(M * N + 64, -9.0, np.float32)
     exact, ks, grid = run_tc(emu, mode, a, b, c, N, 1, a_mn=a_mn, b_mn=b_mn, pair=pair, sms=2, dyn=dyn)
-    assert ks == 1 and grid == 2                 # 4 (2 pair-) tiles on 2 CTAs (1 pair): the persistent loop iterates
+    assert ks == 1 and grid == 2                 # 6 (3 cluster-) tiles on 2 CTAs (1 cluster): the persistent loop iterates
     got = c[:M * N].reshape(M, N)
     assert np.abs(got - exact).max() <= 2e-6 * np.abs(exact).max()
     assert np.all(c[M * N:] == -9.0)
@@ -181,7 +181,7 @@ def test_accumulation_blocks_and_ragged_k(emu, mode, kc, pair):
 @pytest.mark.parametrize("pair,M", [(False, 100), (True, 250)])
 @pytest.mark.parametrize("mode", ["tf32x3", "f16x3"])
 def test_split_k(emu, pair, M, mode):
-    N, K = 200, 1400                             # one output tile, long K: the planner splits K over idle SMs
+    N, K = 120, 1400                             # one output tile, long K: the planner splits K over idle SMs
     a, b = rnd((M, K), 11), rnd((K, N), 12)
     c0 = rnd((M, N), 13)
     c = c0.reshape(-1).copy()
@@ -197,7 +197,7 @@ def test_split_k_of_the_last_partial_wave(emu, pair, mode, dyn, ccol):
     """more tiles than persistent CTAs (pairs), the remainder at most half a wave: the full waves are computed directly, the
     tiles of the remainder as K-ranges through the workspace + reduce kernel (tc_params.h), alpha / beta / bias on both"""
     tile_m = 256 if pair else 128
-    M, N, K = tile_m + 40, 3 * 256 - 10, 1040         # 2 x 3 = 6 tiles on 4 units: 4 direct, 2 split in two halves of K (>= 512 each)
+    M, N, K = tile_m + 40, 3 * 128 - 10, 1040         # 2 x 3 = 6 tiles on 4 units: 4 direct, 2 split in two halves of K (>= 512 each)
     sms = 8 if pair else 4
     a, b = rnd((M, K), 21), rnd((K, N), 22)
     c0 = rnd((M, N), 23)
@@ -221,21 +221,21 @@ def test_split_k_of_the_last_partial_wave(emu, pair, mode, dyn, ccol):
 
 @pytest.mark.parametrize("pair", [False, True])
 @pytest.mark.parametrize("mode", ["f16x3", "tf32x1"])
-def test_c_through_tma_stores_equals_plain_stores(emu, pair, mode):
-    """fp32 C with unit column stride and 16-byte aligned rows leaves through shared-memory staging + cp.async.bulk.tensor
-    stores (32 x 32 boxes, rows past M and columns past N clipped by the copy engine); bit-identical to the plain-store
-    epilogue, C beyond the view untouched, beta / bias / activation included; a padded C (ldc > N) too"""
-    M, N, K = 300, 520, 96                       # ragged rows; the last column block (8 columns) takes the scalar path
+def test_padded_c_equals_compact_c(emu, pair, mode):
+    """fp32 C with a row pitch ldc > N (vector stores of column pairs, ragged rows and a ragged last column block): every
+    element bit-identical to the same product into a compact C (ldc = N), the padding of C untouched, beta / bias /
+    activation included"""
+    M, N, K = 300, 520, 96                       # ragged rows; the last column block (8 of 128 columns) is ragged
     a, b = rnd((M, K), 31), rnd((K, N), 32)
     ldc = N + 8
     c0 = rnd((M, ldc), 33)
     bias = rnd((N,), 34)
     outs = []
-    for c_tma in (1, 0):
-        buf = c0.reshape(-1).copy()
-        exact, _, _ = run_tc(emu, mode, a, b, buf, ldc, 1, alpha=0.5, beta=2.0, pair=pair, sms=4, epi=(bias, 0, 1), c_tma=c_tma)
-        outs.append(buf.reshape(M, ldc))
-    assert np.array_equal(outs[0], outs[1])
+    for pitch in (ldc, N):
+        buf = np.ascontiguousarray(c0[:, :pitch]).reshape(-1).copy()
+        exact, _, _ = run_tc(emu, mode, a, b, buf, pitch, 1, alpha=0.5, beta=2.0, pair=pair, sms=4, epi=(bias, 0, 1))
+        outs.append(buf.reshape(M, pitch))
+    assert np.array_equal(outs[0][:, :N], outs[1])
     assert np.array_equal(outs[0][:, N:], c0[:, N:])                 # the padding of C is not written
     want = np.maximum(0.5 * exact + 2.0 * c0[:, :N] + bias[None, :], 0.0)
     assert np.abs(outs[0][:, :N] - want).max() <= (2e-3 if mode == "tf32x1" else 3e-6) * np.abs(want).max()
@@ -243,7 +243,7 @@ def test_c_through_tma_stores_equals_plain_stores(emu, pair, mode):
 
 @pytest.mark.parametrize("raster", [1, 2, 16])
 def test_raster_groups_cover_every_tile_once(emu, raster):
-    M, N, K = 600, 520, 32                       # 5 x 3 tiles of 128 x 256 on 4 persistent CTAs
+    M, N, K = 600, 520, 32                       # 5 x 5 tiles of 128 x 128 on 4 persistent CTAs
     a, b = rnd((M, K), 14), rnd((K, N), 15)
     c = np.full(M * N, np.nan, np.float32)
     exact, _, grid = run_tc(emu, "tf32x1", a, b, c, N, 1, raster=raster, sms=4)

@@ -3,9 +3,7 @@ oracle: transposes / NCHW<->NHWC (swapaxes.nim:16-112), im2col convolution
 (conv2d_im2col.nim:44-166, the reference's conv known-answer vectors conv2d_common.nim:128-283),
 batched GEMM, copyFrom and forEach on strided views (initialization.nim:80-112, foreach.nim:229-251).
 
-These kernels were written after the round's GPU budget was spent, so their first run on a B200 is the
-round-end run of this file (which sorts after the validated GPU test files for that reason).  Before that they were
-checked as far as a machine without a GPU allows: the kernel source runs on CPU threads against the
+Besides this file, the kernels are checked as far as a machine without a GPU allows: the kernel source runs on CPU threads against the
 oracle (tests/test_emulated_kernels.py), the host side of the entry points too
 (tests/test_emulated_layers_host.py), and this very file runs on the CPU against a stand-in library
 (LASER_B200_EMU=1, tests/test_emulated_python_mirror.py), which checks the Python mirror and the
@@ -90,8 +88,6 @@ def conv_ref(inp, ishape, ker, kshape, padding, strides):
 @pytest.mark.parametrize("N,NR,NC", [(1, 1, 1), (1, 64, 64), (1, 4000, 2000), (3, 33, 70), (2, 68, 132),
                                      (1, 5, 4099), (16, 3, 224 * 224), (1, 8192, 8192)])
 def test_transpose_dev(esz, N, NR, NC):
-    if esz == 8 and NR * NC > 4000 * 2000:
-        pytest.skip("large case covered at 4 bytes")
     cpu_budget(N * NR * NC)
     dt = NP_OF[esz]
     src = (np.arange(N * NR * NC, dtype=np.int64) * 2654435761 % 65521).astype(dt)

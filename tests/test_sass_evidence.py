@@ -1,6 +1,6 @@
-"""CPU-only: the shipped library really is a tcgen05 / TMEM / TMA build (the SASS mnemonics of B200_PROFILING.md's
-"what proves a Blackwell-native kernel" table), for every tensor-core kernel family, and holds no legacy tensor path.
-`python tests/test_sass_evidence.py` rewrites the excerpt committed under profiles/."""
+"""CPU-only: the shipped library really is a wgmma / TMA / mbarrier build (HGMMA = wgmma.mma_async, UTMALDG = TMA tile
+load, SYNCS = mbarrier, USETMAXREG = setmaxnreg), for every tensor-core kernel family, and holds no mma.sync half-precision
+path.  `python tests/test_sass_evidence.py DIR` writes the per-kernel counts to DIR/sass_mnemonics.txt."""
 import collections
 import os
 import re
@@ -12,8 +12,7 @@ import pytest
 import laser_b200 as L
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-MNEMONICS = ("UTCHMMA", "UTCBAR", "LDTM", "UTMALDG", "UTMASTG", "UBLKCP", "LDGSTS", "DMMA", "HMMA", "HGMMA", "ATOMG", "SYNCS", "STG.E.128",
-             "USETMAXREG")
+MNEMONICS = ("HGMMA", "WARPGROUP", "UTMALDG", "UBLKCP", "LDGSTS", "DMMA", "HMMA", "ATOMG", "SYNCS", "STG.E.128", "USETMAXREG")
 
 
 import functools
@@ -42,15 +41,16 @@ def sass_counts():
     return res
 
 
-def test_tensor_core_kernels_are_tcgen05_tmem_tma():
+def test_tensor_core_kernels_are_wgmma_tma():
     counts = sass_counts()
     tc = {k: v for k, v in counts.items() if "gemm_tc_kernel" in k}
-    assert len(tc) == 32, sorted(tc)            # 4 families x (A, B major-ness) x (single CTA, CTA pair)
+    # 16-bit families (bf16, f16x3): 4 operand major-nesses x (single CTA, cluster of two); tf32 families: K-major only x 2
+    assert len(tc) == 2 * 4 * 2 + 2 * 2, sorted(tc)
     for k, c in tc.items():
-        assert c["UTCHMMA"] >= 4 and c["LDTM"] >= 8 and c["UTMALDG"] >= 2 and c["UTCBAR"] >= 2, (k, dict(c))
+        assert c["HGMMA"] >= 4 and c["WARPGROUP"] >= 2 and c["UTMALDG"] >= 2 and c["SYNCS"] >= 2, (k, dict(c))
         assert c["USETMAXREG"] == 2, k          # warp-specialised register split
     for k, c in counts.items():
-        assert c["HMMA"] == 0 and c["HGMMA"] == 0, k       # no half-precision mma.sync / wgmma anywhere in the library
+        assert c["HMMA"] == 0, k                # no half-precision mma.sync anywhere in the library
 
 
 def test_fp64_tensor_cores_and_bulk_copies():
@@ -62,11 +62,13 @@ def test_fp64_tensor_cores_and_bulk_copies():
 
 
 if __name__ == "__main__":
+    import sys
     counts = sass_counts()
-    with open(os.path.join(ROOT, "profiles", "r02_sass_mnemonics.txt"), "w") as f:
-        f.write("# cuobjdump -sass laser_b200/lib/liblaser_b200.so: occurrences of the Blackwell mnemonics per tensor-core kernel\n")
-        f.write("# (UTCHMMA = tcgen05.mma, LDTM = tcgen05.ld, UTMALDG = cp.async.bulk.tensor load, UTCBAR = tcgen05.commit, UBLKCP = cp.async.bulk,\n# LDGSTS = cp.async, DMMA = mma.sync.f64)\n")
+    out_dir = sys.argv[1] if len(sys.argv) > 1 else "."
+    with open(os.path.join(out_dir, "sass_mnemonics.txt"), "w") as f:
+        f.write("# cuobjdump -sass laser_b200/lib/liblaser_b200.so: occurrences per tensor-core kernel\n")
+        f.write("# (HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / wait, UTMALDG = cp.async.bulk.tensor load, UBLKCP = cp.async.bulk,\n# LDGSTS = cp.async, SYNCS = mbarrier, DMMA = mma.sync.f64)\n")
         for k in sorted(counts):
             if "gemm_tc_kernel" in k or "gemm_dmma_kernel" in k or "f16x2_rows_ring_kernel" in k:
                 f.write("%s\n    %s\n" % (k, "  ".join("%s=%d" % (m, counts[k][m]) for m in MNEMONICS if counts[k][m])))
-    print("wrote profiles/r02_sass_mnemonics.txt")
+    print("wrote", os.path.join(out_dir, "sass_mnemonics.txt"))

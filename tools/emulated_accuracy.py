@@ -1,6 +1,6 @@
 """Error of every fp32 tensor-core mode against an fp64 product, on the HOST-EMULATED library (tests/emu): operand
 splitting, pass order and the kc-blocked summation are the product's; the accumulator inside a block is a plain fp32
-FMA chain, NOT the tensor core's truncating one (that part is what tools/accuracy_probe.py measures on a B200).
+FMA chain, NOT the tensor core's truncating one (that part is what tools/accuracy_probe.py measures on an H100).
   LASER_B200_LIB=tests/emu/_build/liblaser_b200_hostemu.so LASER_B200_EMU=1 python tools/emulated_accuracy.py [M N K]
 """
 import sys, numpy as np

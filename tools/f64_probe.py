@@ -1,4 +1,4 @@
-"""fp64 GEMM on one B200: the tensor-core (DMMA) kernel against the CUDA-core kernel, TFLOP/s and bit-equality of the two.
+"""fp64 GEMM on one H100: the tensor-core (DMMA) kernel against the CUDA-core kernel, TFLOP/s and bit-equality of the two.
     python tools/f64_probe.py [n ...]"""
 import os, subprocess, sys, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

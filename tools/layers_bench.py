@@ -1,4 +1,4 @@
-"""Timing of the steps either side of the GEMM on one B200 (HBM roofline), at the reference's own
+"""Timing of the steps either side of the GEMM on one H100 (HBM roofline), at the reference's own
 bench shapes: transpose 4000x2000 f32 (benchmarks/transpose/transpose_bench.nim:54-55; the
 reference's best CPU variant: 9.2 ms = 0.78 GMEMOP/s), NCHW<->NHWC, im2col and conv2d_im2col on
 16x3x224x224 with 20 3x3 filters (benchmarks/convolution/conv2d_bench.nim:52-62).

@@ -1,4 +1,4 @@
-"""Interleaved A/B timing (the B200 is power-capped: sequential blocks of runs are not comparable)."""
+"""Interleaved A/B timing (the GPU may be power-capped: sequential blocks of runs are not comparable)."""
 import os, sys, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, laser_b200 as L

@@ -1,4 +1,4 @@
-"""Time and error of one fp32 tensor-core mode (f16x3 | tf32x3 | tf32x1) next to tf32x3 on one B200 -> one JSON line on stdout.
+"""Time and error of one fp32 tensor-core mode (f16x3 | tf32x3 | tf32x1) next to tf32x3 on one H100 -> one JSON line on stdout.
 
 bench.py runs this in a CHILD process per mode (with a timeout) after all of its own measurements: the modes were written
 after the round's GPU minutes were spent, so their first run on silicon must not be able to take the bench line down.
