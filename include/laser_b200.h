@@ -171,6 +171,37 @@ int laser_b200_gemm_strided_f32_epi_dev(int64_t M, int64_t N, int64_t K, float a
                                         float beta, float *C, int64_t rowStrideC, int64_t colStrideC,
                                         const laser_b200_epilogue *epi, int path, void *stream);
 
+/* ---- fused prologue ------------------------------------------------------
+ * C <- act(alpha * opA(A) * opB(B) + beta * C + bias): an elementwise op applied to an operand while it is prepared for the
+ * GEMM, so op(A) / op(B) is never written to memory.  The reference plans this as the second half of its "Operation fusion"
+ * roadmap: fuse operations during the prepacking, for backward propagation, where the derivatives of relu, tanh and sigmoid
+ * come before each matrix multiplication (README.md:244-245).  Typical calls: dX = (dY . relu'(Z)) * W^T (op on A) and
+ * dW = X^T * (dY . tanh'(Y)) (op on B).
+ *   ops 1-3 use the formulas of the epilogue's activations; ops 4-6 read `aux` (same extents as the operand:
+ *   A: M x K, B: K x N, any element strides) and round every operation separately, in the order shown, without contraction.
+ *   RELU_GRAD is a select: z <= 0 or NaN gives 0 even for x = inf.
+ * opA, opB, epi: NULL (or op NONE) = no op; with all three NULL the call is laser_b200_gemm_strided_f32_dev.  An unknown op,
+ * or a derivative op without aux, returns LASER_B200_EINVAL before anything is launched.  aux is read only and may alias its
+ * operand; like A and B it must not alias C.  PATH_AUTO never takes the N <= 4 GEMV shortcut for a call with an op. */
+#define LASER_B200_OP_NONE 0
+#define LASER_B200_OP_RELU 1          /* x -> fmaxf(x, 0)                 */
+#define LASER_B200_OP_TANH 2          /* x -> tanhf(x)                    */
+#define LASER_B200_OP_SIGMOID 3       /* x -> 1 / (1 + expf(-x))          */
+#define LASER_B200_OP_RELU_GRAD 4     /* x -> (z > 0) ? x : 0             z = aux element (pre-activation, or relu output) */
+#define LASER_B200_OP_TANH_GRAD 5     /* x -> x * (1 - y*y)               y = aux element (the tanh output) */
+#define LASER_B200_OP_SIGMOID_GRAD 6  /* x -> x * (y * (1 - y))           y = aux element (the sigmoid output) */
+typedef struct {
+  int32_t op;
+  const float *aux;                   /* device; NULL for ops 0-3 */
+  int64_t auxRowStride, auxColStride; /* element strides of aux, any int64 */
+} laser_b200_operand_op;
+int laser_b200_gemm_strided_f32_fused_dev(int64_t M, int64_t N, int64_t K, float alpha,
+                                          const float *A, int64_t rowStrideA, int64_t colStrideA,
+                                          const float *B, int64_t rowStrideB, int64_t colStrideB,
+                                          float beta, float *C, int64_t rowStrideC, int64_t colStrideC,
+                                          const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
+                                          const laser_b200_epilogue *epi, int path, void *stream);
+
 /* ---- pre-packed operands (device) -----------------------------------------
  * Replaces  gemm_prepackA_mem_required / gemm_prepackB_mem_required, gemm_prepackA / gemm_prepackB
  * and gemm_packed   (laser/primitives/matrix_multiplication/gemm_prepacked.nim:63-292).

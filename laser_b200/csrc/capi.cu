@@ -430,9 +430,11 @@ enum SplitMode {
 
 // F16X3 preparation of a row-contiguous fp32 operand [R][Cc] (mn along R, or along Cc when the operand is MN-major):
 // K-major: ONE fused pass (abs-max per row, scale, split; split.cuh).  MN-major: the scale belongs to a column, so the
-// abs-max pass (strip reduction + atomicMax) comes first and the split second.
+// abs-max pass (strip reduction + atomicMax) comes first and the split second.  HAS_OP: both passes apply `op` on load, so
+// the scale words are those of the op's output.  The ring kernel has no op variant: long op'd rows take the register kernel.
+template <bool HAS_OP>
 int f16x2_prepare(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, bool mn_along_cols, const OperandWs &w,
-                  int64_t ld_b, cudaStream_t s) {
+                  int64_t ld_b, cudaStream_t s, const OperandOp &op) {
   uint32_t *words = static_cast<uint32_t *>(c.f16s.ptr) + w.amax_off;
   const int64_t n_mn = mn_along_cols ? Cc : R;
   if (c.f16s.bytes < static_cast<size_t>(w.amax_off + n_mn) * sizeof(uint32_t))
@@ -441,14 +443,14 @@ int f16x2_prepare(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_l
   if (mn_along_cols) {
     CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(n_mn) * sizeof(uint32_t), s));
     const int64_t items = ((Cc + 3) / 4) * ((R + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS);
-    absmax_mn_kernel<true><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(src, R, Cc, src_ld, words);
+    absmax_mn_kernel<true, HAS_OP><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(src, R, Cc, src_ld, words, op);
     COUNT_LAUNCH();
     CHECK_LAUNCH();
     const int64_t split_items = ((Cc + 255) / 256) * ((R + SPLIT_ROWS - 1) / SPLIT_ROWS);
-    split_rows_f16x2_kernel<true><<<grid_for(c, split_items, 8), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words);
+    split_rows_f16x2_kernel<true, HAS_OP><<<grid_for(c, split_items, 8), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words, op);
   } else if (Cc <= 4 * 32 * F16ROWS_MAXV) {   // short rows: a warp per row
-    f16x2_rows_fused_kernel<32><<<grid_for(c, (R + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words);
-  } else if (c.prep_ring && f16x2_rows_ring_ok(src, Cc, src_ld)) {   // rows prefetched into a shared-memory ring by the copy engine
+    f16x2_rows_fused_kernel<32, HAS_OP><<<grid_for(c, (R + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words, op);
+  } else if (!HAS_OP && c.prep_ring && f16x2_rows_ring_ok(src, Cc, src_ld)) {   // rows prefetched into a shared-memory ring by the copy engine
     const size_t smem = f16x2_rows_ring_smem(Cc);
     if (!c.ring_attr_set) {
       CUDA_TRY(cudaFuncSetAttribute(f16x2_rows_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -457,7 +459,7 @@ int f16x2_prepare(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_l
     }
     f16x2_rows_ring_kernel<<<grid_for(c, R, 2), 256, smem, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words);
   } else {
-    f16x2_rows_fused_kernel<256><<<grid_for(c, R, 4), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words);
+    f16x2_rows_fused_kernel<256, HAS_OP><<<grid_for(c, R, 4), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words, op);
   }
   COUNT_LAUNCH();
   CHECK_LAUNCH();
@@ -469,7 +471,7 @@ int f16x2_prepare(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_l
 int f16x2_absmax_cols(Ctx &c, const float *B, int64_t K, int64_t N, int64_t ld, uint32_t *words, cudaStream_t s) {
   CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(N) * sizeof(uint32_t), s));
   const int64_t items = ((N + 3) / 4) * ((K + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS);
-  absmax_mn_kernel<true><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(B, K, N, ld, words);
+  absmax_mn_kernel<true><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(B, K, N, ld, words, OperandOp());
   COUNT_LAUNCH();
   CHECK_LAUNCH();
   return LASER_B200_OK;
@@ -481,9 +483,9 @@ int f16x2_prepare_panel(Ctx &c, bool row_major, const float *Bp, int64_t K, int6
                         uint32_t *words, cudaStream_t s) {
   if (row_major) {
     const int64_t split_items = ((w + 255) / 256) * ((K + SPLIT_ROWS - 1) / SPLIT_ROWS);
-    split_rows_f16x2_kernel<true><<<grid_for(c, split_items, 8), 256, 0, s>>>(Bp, K, w, ld, hi, lo, w, words);
+    split_rows_f16x2_kernel<true><<<grid_for(c, split_items, 8), 256, 0, s>>>(Bp, K, w, ld, hi, lo, w, words, OperandOp());
   } else if (K <= 4 * 32 * F16ROWS_MAXV) {
-    f16x2_rows_fused_kernel<32><<<grid_for(c, (w + 7) / 8, 4), 256, 0, s>>>(Bp, w, K, ld, hi, lo, K, words);
+    f16x2_rows_fused_kernel<32><<<grid_for(c, (w + 7) / 8, 4), 256, 0, s>>>(Bp, w, K, ld, hi, lo, K, words, OperandOp());
   } else if (c.prep_ring && f16x2_rows_ring_ok(Bp, K, ld)) {
     if (!c.ring_attr_set) {
       CUDA_TRY(cudaFuncSetAttribute(f16x2_rows_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -492,20 +494,52 @@ int f16x2_prepare_panel(Ctx &c, bool row_major, const float *Bp, int64_t K, int6
     }
     f16x2_rows_ring_kernel<<<grid_for(c, w, 2), 256, f16x2_rows_ring_smem(K), s>>>(Bp, w, K, ld, hi, lo, K, words);
   } else {
-    f16x2_rows_fused_kernel<256><<<grid_for(c, w, 4), 256, 0, s>>>(Bp, w, K, ld, hi, lo, K, words);
+    f16x2_rows_fused_kernel<256><<<grid_for(c, w, 4), 256, 0, s>>>(Bp, w, K, ld, hi, lo, K, words, OperandOp());
   }
   COUNT_LAUNCH();
   CHECK_LAUNCH();
   return LASER_B200_OK;
 }
 
+// Operand ops of the fused-prologue entry.  Host side, `OperandOp` describes aux as [mn][k] like its Operand
+// (aux_sr = s_mn, aux_sc = s_k); the preparation kernels see it over their [R][Cc] rows, where R runs along k when the
+// prepared layout is MN-major.
+inline OperandOp kernel_op(const OperandOp &op, bool rows_along_k) {
+  OperandOp k = op;
+  if (rows_along_k) { k.aux_sr = op.aux_sc; k.aux_sc = op.aux_sr; }
+  return k;
+}
+// aux can be read at the operand's own offsets by the row kernels
+inline bool op_same_layout(const Operand &o, const OperandOp &op) {
+  return !op.aux || (op.aux_sr == o.s_mn && op.aux_sc == o.s_k && (reinterpret_cast<uintptr_t>(op.aux) & 15) == 0);
+}
+// op(operand) gathered into a compact fp32 [mn][round_up(k, 4)] array (aux read with its own strides)
+int gather_op(Ctx &c, const Operand &o, const OperandOp &op, Buffer &dst, cudaStream_t s, const float **out) {
+  const int64_t ld = round_up(o.k, 4);
+  int rc;
+  if ((rc = ensure(dst, static_cast<size_t>(o.mn) * ld * sizeof(float)))) return rc;
+  const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32);
+  const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
+  pack_general_kernel<float, 0, true><<<grid_for(c, tiles, 8), 256, 0, s>>>(static_cast<const float *>(o.ptr), o.mn, o.k, o.s_mn,
+                                                                           o.s_k, static_cast<float *>(dst.ptr), nullptr, ld,
+                                                                           read_along_r, op);
+  COUNT_LAUNCH();
+  CHECK_LAUNCH();
+  *out = static_cast<const float *>(dst.ptr);
+  return LASER_B200_OK;
+}
+
+// op: nullptr, or an operand op (fp32 operands only)
 template <int ESZ>
 int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w, int block_mn,
-                    OperandMaps *m, bool *used_ws, cudaStream_t s) {
+                    OperandMaps *m, bool *used_ws, cudaStream_t s, const OperandOp *op = nullptr) {
   using ET = typename std::conditional<ESZ == 4, float, uint16_t>::type;
   // wgmma reads tf32 tiles K-major only: an MN-major fp32 operand of the tf32 modes is gathered into compact K-major rows
   const Major mj0 = classify(o, ESZ);
-  const Major mj = (ESZ == 4 && mode != SPLIT_F16X2 && mj0 == MN_MAJOR) ? GENERAL : mj0;
+  Major mj = (ESZ == 4 && mode != SPLIT_F16X2 && mj0 == MN_MAJOR) ? GENERAL : mj0;
+  // an op is applied on load by the preparation kernels when aux has the operand's layout; otherwise, and when TMA would
+  // read the caller's memory as it is (SPLIT_NONE), one gather applies it
+  if (op && mj != GENERAL && (mode == SPLIT_NONE || !op_same_layout(o, *op))) mj = GENERAL;
   const int64_t vec = 16 / ESZ;
   int rc;
   if (mj != GENERAL && mode == SPLIT_NONE) {
@@ -532,7 +566,10 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
       if ((rc = ensure(*w.p1, bytes_b))) return rc;
       const float *src = static_cast<const float *>(o.ptr);
       int64_t src_ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;
-      if (mj == GENERAL) {
+      if (mj == GENERAL && op) {   // the op applied by the gather; what follows is the plain preparation of its output
+        if ((rc = gather_op(c, o, *op, *w.gather, s, &src))) return rc;
+        src_ld = ld;
+      } else if (mj == GENERAL) {
         // general strides: one coalesced gather into a compact fp32 array (the surviving descendant of pack_A / pack_B),
         // then the fused scale + split of that
         if ((rc = ensure(*w.gather, bytes))) return rc;
@@ -540,13 +577,16 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
         const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
         pack_general_kernel<float, 0><<<grid_for(c, tiles, 8), 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k,
                                                                             static_cast<float *>(w.gather->ptr), nullptr, ld,
-                                                                            read_along_r);
+                                                                            read_along_r, OperandOp());
         COUNT_LAUNCH();
         CHECK_LAUNCH();
         src = static_cast<const float *>(w.gather->ptr);
         src_ld = ld;
       }
-      if ((rc = f16x2_prepare(c, src, R, Cc, src_ld, out_mj == MN_MAJOR, w, ld_b, s))) return rc;
+      rc = (op && mj != GENERAL)
+               ? f16x2_prepare<true>(c, src, R, Cc, src_ld, out_mj == MN_MAJOR, w, ld_b, s, kernel_op(*op, out_mj == MN_MAJOR))
+               : f16x2_prepare<false>(c, src, R, Cc, src_ld, out_mj == MN_MAJOR, w, ld_b, s, OperandOp());
+      if (rc) return rc;
       if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, o.k, ld_b, block_mn))) return rc;
       return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, o.k, ld_b, block_mn);
     }
@@ -558,8 +598,13 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
     if constexpr (ESZ == 4) {
       const int64_t src_ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;
       const int64_t items = R * ((Cc + 3) / 4);
-      split_rows_tf32_kernel<<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
-          static_cast<const float *>(o.ptr), R, Cc, src_ld, static_cast<float *>(w.p0->ptr), static_cast<float *>(w.p1->ptr), ld);
+      float *hi = static_cast<float *>(w.p0->ptr), *lo = static_cast<float *>(w.p1->ptr);
+      if (op)
+        split_rows_tf32_kernel<true><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
+            static_cast<const float *>(o.ptr), R, Cc, src_ld, hi, lo, ld, kernel_op(*op, mj == MN_MAJOR));
+      else
+        split_rows_tf32_kernel<false><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
+            static_cast<const float *>(o.ptr), R, Cc, src_ld, hi, lo, ld, OperandOp());
     }
   } else {
     const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32);
@@ -568,13 +613,17 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
     const ET *src = static_cast<const ET *>(o.ptr);
     ET *d0 = static_cast<ET *>(w.p0->ptr);
     if constexpr (ESZ == 4) {
-      if (mode == SPLIT_TF32)
-        pack_general_kernel<float, 1><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, static_cast<float *>(w.p1->ptr),
-                                                           ld, read_along_r);
+      float *d1 = static_cast<float *>(w.p1->ptr);
+      if (mode == SPLIT_TF32 && op)
+        pack_general_kernel<float, 1, true><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, *op);
+      else if (mode == SPLIT_TF32)
+        pack_general_kernel<float, 1><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, OperandOp());
+      else if (op)
+        pack_general_kernel<float, 0, true><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r, *op);
       else
-        pack_general_kernel<float, 0><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r);
+        pack_general_kernel<float, 0><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r, OperandOp());
     } else {
-      pack_general_kernel<ET, 0><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r);
+      pack_general_kernel<ET, 0><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r, OperandOp());
     }
   }
   COUNT_LAUNCH();
@@ -674,9 +723,11 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
 template <int SRC_ESZ, typename OutT>
 int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, const void *A, int64_t rsA,
             int64_t csA, const void *B, int64_t rsB, int64_t csB, float beta, OutT *C, int64_t rsC,
-            int64_t csC, cudaStream_t s, const Epilogue &epi, cudaEvent_t b_ready = nullptr) {
+            int64_t csC, cudaStream_t s, const Epilogue &epi, cudaEvent_t b_ready = nullptr, const OperandOp *opA = nullptr,
+            const OperandOp *opB = nullptr) {
   // b_ready: B becomes valid only when this event has fired (the row-sharded driver: B is in flight on the communication
-  // stream); everything that does not read B -- the preparation of A -- is queued before the wait
+  // stream); everything that does not read B -- the preparation of A -- is queued before the wait.
+  // opA / opB: operand ops applied while the operands are prepared (fp32 only)
   if (M > 0x7fffffffLL || N > 0x7fffffffLL || K > 0x7fffffffLL)
     return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: extents must fit in int32");
   std::lock_guard<std::mutex> lk(c.mu);  // workspace + descriptor construction are per context
@@ -693,12 +744,12 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   if (rc) return rc;
   int64_t f16_b_off = 0;
   if (mode == SPLIT_F16X2 && (rc = f16_scales(c, M, N, &f16_b_off))) { prof_abort(c, &ep); return rc; }
-  rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s);
+  rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s, opA);
   if (rc) { prof_abort(c, &ep); return rc; }
   // clusters of two CTAs (256 x 128 tiles) when enabled and there are at least two 128-row blocks
   const bool pair = c.cta_pair && M > TC_BLOCK_M;
   if (b_ready) CUDA_TRY(cudaStreamWaitEvent(s, b_ready, 0));
-  rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, s);
+  rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, s, opB);
   if (rc) { prof_abort(c, &ep); return rc; }
   const int prep_launches = static_cast<int>(g_launches.load() - launches_before);
   rc = prof_close(c, s, &ep, prep_launches);
@@ -764,16 +815,16 @@ int prepack_dev(int which, void *dst, int64_t mn, int64_t k, const float *src, i
       const int64_t tiles = ((mn + 31) / 32) * ((k + 31) / 32);
       const int read_along_r = (llabs(s_mn) < llabs(s_k)) ? 1 : 0;
       pack_general_kernel<float, 0><<<grid_for(*c, tiles, 8), 256, 0, s>>>(src, mn, k, s_mn, s_k, static_cast<float *>(g.ptr),
-                                                                           nullptr, ld, read_along_r);
+                                                                           nullptr, ld, read_along_r, OperandOp());
       COUNT_LAUNCH();
       CHECK_LAUNCH();
       rows = static_cast<const float *>(g.ptr);
       rows_ld = ld;
     }
     if (k <= 4 * 32 * F16ROWS_MAXV)
-      f16x2_rows_fused_kernel<32><<<grid_for(*c, (mn + 7) / 8, 4), 256, 0, s>>>(rows, mn, k, rows_ld, h, l, L.ld_b, amax);
+      f16x2_rows_fused_kernel<32><<<grid_for(*c, (mn + 7) / 8, 4), 256, 0, s>>>(rows, mn, k, rows_ld, h, l, L.ld_b, amax, OperandOp());
     else
-      f16x2_rows_fused_kernel<256><<<grid_for(*c, mn, 4), 256, 0, s>>>(rows, mn, k, rows_ld, h, l, L.ld_b, amax);
+      f16x2_rows_fused_kernel<256><<<grid_for(*c, mn, 4), 256, 0, s>>>(rows, mn, k, rows_ld, h, l, L.ld_b, amax, OperandOp());
     COUNT_LAUNCH();
     CHECK_LAUNCH();
     CUDA_TRY(cudaEventRecord(c->ws_free, s));
@@ -860,14 +911,14 @@ inline bool is_tc_mode(int mode) {
 //   work <= 128^3 (the reference's own switch, gemm.nim:140-141): exact kernel -- a 128 x 256 tensor-core tile would be
 //       mostly padding;
 //   mode SIMT: exact kernel for every shape (the mode documented as bit-identical to the CPU reference), before any shortcut;
-//   N <= 4 tall problems without a fused epilogue: warp-shuffle GEMV (-1);
+//   N <= 4 tall problems without a fused epilogue or operand op: warp-shuffle GEMV (-1);
 //   otherwise the fp32 mode in force.
-int resolve_auto(int64_t M, int64_t N, int64_t K, const Epilogue &epi) {
+int resolve_auto(int64_t M, int64_t N, int64_t K, const Epilogue &epi, bool operand_op = false) {
   const double work = static_cast<double>(M) * N * K;
   if (work <= 128.0 * 128.0 * 128.0) return LASER_B200_PATH_SIMT;
   const int mode = g_f32_mode.load();
   if (mode == LASER_B200_PATH_SIMT) return LASER_B200_PATH_SIMT;
-  if (N <= 4 && M >= 1024 && !epi.bias && !epi.act) return -1;
+  if (N <= 4 && M >= 1024 && !epi.bias && !epi.act && !operand_op) return -1;
   // few output rows, wide N (the im2col convolution's product): the exact few-rows kernel streams B once; a tensor-core
   // call would first spend three passes over B preparing it and then compute 84+ % padding (20 x 788544 x 27: 0.08 ms
   // against 0.28 ms, profiles/r02_large_shapes.txt) -- and exact is at least as accurate as any tensor-core mode
@@ -875,17 +926,42 @@ int resolve_auto(int64_t M, int64_t N, int64_t K, const Epilogue &epi) {
   return mode < 0 ? kDefaultF32Mode : mode;
 }
 
+// Exact path with operand ops: each op'd operand is materialised once by the gather (compact [mn][k] workspace) and the
+// unchanged exact kernel multiplies that, so the path stays bit-identical to the CPU reference on the op'd operands.
+int gemm_simt_ops(Ctx &c, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
+                  const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC, cudaStream_t s,
+                  const Epilogue &epi, const OperandOp *opA, const OperandOp *opB) {
+  std::lock_guard<std::mutex> lk(c.mu);   // the gather buffers are workspace
+  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
+  int rc;
+  if (opA) {
+    if ((rc = gather_op(c, Operand{A, M, K, rsA, csA}, *opA, c.gather[0], s, &A))) return rc;
+    rsA = round_up(K, 4); csA = 1;
+  }
+  if (opB) {
+    if ((rc = gather_op(c, Operand{B, N, K, csB, rsB}, *opB, c.gather[1], s, &B))) return rc;
+    rsB = 1; csB = round_up(K, 4);
+  }
+  if ((rc = gemm_simt<float>(c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi))) return rc;
+  CUDA_TRY(cudaEventRecord(c.ws_free, s));
+  return LASER_B200_OK;
+}
+
+// opA / opB: operand ops of the fused-prologue entry (nullptr: none)
 int f32_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
             const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
-            int path, void *stream, const Epilogue &epi = Epilogue(), cudaEvent_t b_ready = nullptr) {
+            int path, void *stream, const Epilogue &epi = Epilogue(), cudaEvent_t b_ready = nullptr,
+            const OperandOp *opA = nullptr, const OperandOp *opB = nullptr) {
   int rc = check_args(M, N, K, A, B, C);
   if (rc == -1) return LASER_B200_OK;
   if (rc) return rc;
+  const bool has_op = opA || opB;
+  if (has_op && path == -1) return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
   Ctx *c;
   rc = get_ctx(&c);
   if (rc) return rc;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, K, epi);
+  if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, K, epi, has_op);
   if (b_ready && !is_tc_mode(path)) CUDA_TRY(cudaStreamWaitEvent(s, b_ready, 0));   // no separate preparation of A to overlap
   switch (path) {
     case -1: {
@@ -913,7 +989,8 @@ int f32_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_
       break;
     }
     case LASER_B200_PATH_SIMT:
-      rc = gemm_simt<float>(*c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi);
+      if (has_op) rc = gemm_simt_ops(*c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, opA, opB);
+      else rc = gemm_simt<float>(*c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi);
       if (rc) return rc;
       g_last_path = LASER_B200_PATH_SIMT;
       break;
@@ -922,7 +999,8 @@ int f32_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_
     case LASER_B200_PATH_F16X3:
       // F16X3 (default): two fp16 pieces of each operand scaled by a power of two per row of A / column of B (device-side
       // abs-max), three passes, the epilogue undoes the scales.  TF32X3: hi/lo tf32 pieces, three passes.  TF32X1: one pass.
-      rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, b_ready);
+      rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, b_ready,
+                             opA, opB);
       if (rc) return rc;
       g_last_path = path;
       break;
@@ -963,6 +1041,31 @@ int bf16_dev(int64_t M, int64_t N, int64_t K, float alpha, const uint16_t *A, in
   if (rc) return rc;
   g_last_path = LASER_B200_PATH_BF16;
   return finish(*c, static_cast<cudaStream_t>(stream), s);
+}
+
+// arguments of the fused entries -> their internal form; nothing is launched before both are validated
+int epilogue_of(const laser_b200_epilogue *epi, Epilogue *e) {
+  if (!epi) return LASER_B200_OK;
+  if (epi->activation < 0 || epi->activation > 3) return set_error(LASER_B200_EINVAL, "unknown activation %d", epi->activation);
+  e->bias = epi->bias;
+  e->bias_per_row = epi->bias_per_row ? 1 : 0;
+  e->act = epi->activation;
+  return LASER_B200_OK;
+}
+// *out = nullptr for no op; aux strides become [mn][k] ones (B is seen as [n][k])
+int operand_op_of(const laser_b200_operand_op *in, bool is_b, OperandOp *op, const OperandOp **out) {
+  *out = nullptr;
+  if (!in || in->op == LASER_B200_OP_NONE) return LASER_B200_OK;
+  if (in->op < LASER_B200_OP_NONE || in->op > LASER_B200_OP_SIGMOID_GRAD)
+    return set_error(LASER_B200_EINVAL, "unknown operand op %d", in->op);
+  const bool derivative = in->op >= LASER_B200_OP_RELU_GRAD;
+  if (derivative && !in->aux) return set_error(LASER_B200_EINVAL, "operand op %d needs an aux tensor", in->op);
+  op->op = in->op;
+  op->aux = derivative ? in->aux : nullptr;
+  op->aux_sr = is_b ? in->auxColStride : in->auxRowStride;
+  op->aux_sc = is_b ? in->auxRowStride : in->auxColStride;
+  *out = op;
+  return LASER_B200_OK;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1256,13 +1359,23 @@ int laser_b200_gemm_strided_f32_epi_dev(int64_t M, int64_t N, int64_t K, float a
                                         int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
                                         const laser_b200_epilogue *epi, int path, void *stream) {
   Epilogue e;
-  if (epi) {
-    if (epi->activation < 0 || epi->activation > 3) return set_error(LASER_B200_EINVAL, "unknown activation %d", epi->activation);
-    e.bias = epi->bias;
-    e.bias_per_row = epi->bias_per_row ? 1 : 0;
-    e.act = epi->activation;
-  }
+  const int rc = epilogue_of(epi, &e);
+  if (rc) return rc;
   return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, e);
+}
+int laser_b200_gemm_strided_f32_fused_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A,
+                                          int64_t rsA, int64_t csA, const float *B, int64_t rsB,
+                                          int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
+                                          const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
+                                          const laser_b200_epilogue *epi, int path, void *stream) {
+  Epilogue e;
+  OperandOp oa, ob;
+  const OperandOp *pa, *pb;
+  int rc;
+  if ((rc = epilogue_of(epi, &e))) return rc;
+  if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
+  if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
+  return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, e, nullptr, pa, pb);
 }
 int laser_b200_gemm_strided_f64_dev(int64_t M, int64_t N, int64_t K, double alpha, const double *A,
                                     int64_t rsA, int64_t csA, const double *B, int64_t rsB,

@@ -43,11 +43,65 @@ __device__ __forceinline__ float tf32_lo(float x, float hi) {
   return ((__float_as_uint(hi) & 0x7f800000u) == 0x7f800000u) ? 0.0f : tf32_rna(x - hi);
 }
 
+// ---- prologue fusion: an elementwise op applied to the operand while it is prepared ---------------------------------
+// The kernels below take `template <bool HAS_OP>` (false: the plain kernel, which never reads `op`) and an OperandOp.
+// Element (r, c) of the kernel's [R][Cc] view has its aux element at aux[r * aux_sr + c * aux_sc]; the row kernels read aux
+// with the operand's own offsets (aux_sr = src_ld, aux_sc = 1, 16-byte aligned), the gather with any strides.
+struct OperandOp {
+  int op = 0;                   // LASER_B200_OP_* (1 .. 6)
+  const float *aux = nullptr;   // derivative ops (4 .. 6) only
+  int64_t aux_sr = 0, aux_sc = 0;
+};
+// Ops 1-3: the formulas of the epilogue's activations (gemm_tc.cuh: epi_act).  Ops 4-6: every operation rounded on its
+// own, in the order written (no contraction), so that the exact path is bit-identical to a step-by-step restatement.
+// (tanhf / expf out of line: inlined into every element of the unrolled row kernels they make them spill)
+#ifndef LB200_HOST_EMULATION
+static __device__ __noinline__ float operand_act(int op, float x) {
+#else
+inline float operand_act(int op, float x) {
+#endif
+  return op == 2 ? tanhf(x) : 1.0f / (1.0f + expf(-x));
+}
+__device__ __forceinline__ float operand_op(int op, float x, float y) {
+  switch (op) {
+    case 1: return fmaxf(x, 0.0f);
+    case 2:
+    case 3: return operand_act(op, x);
+    case 4: return y > 0.0f ? x : 0.0f;                               // a select: inf * 0 never happens
+    case 5: return __fmul_rn(x, __fsub_rn(1.0f, __fmul_rn(y, y)));
+    case 6: return __fmul_rn(x, __fmul_rn(y, __fsub_rn(1.0f, y)));
+    default: return x;
+  }
+}
+__device__ __forceinline__ float4 load_row_vec(const float *row, int64_t c, int64_t Cc) {
+  float4 v;
+  if (c + 4 <= Cc) {
+    v = *reinterpret_cast<const float4 *>(row + c);
+  } else {   // ragged end of the row: one to three elements
+    v.x = row[c];
+    v.y = (c + 1 < Cc) ? row[c + 1] : 0.0f;
+    v.z = (c + 2 < Cc) ? row[c + 2] : 0.0f;
+    v.w = 0.0f;
+  }
+  return v;
+}
+// the op on four consecutive elements c .. c+3 of row r (v: the operand's values, 0 past Cc); elements past Cc stay 0 (they
+// are the padding of the prepared arrays)
+__device__ __forceinline__ float4 op_vec(const OperandOp &op, float4 v, int64_t r, int64_t c, int64_t Cc) {
+  const float4 y = op.aux ? load_row_vec(op.aux + r * op.aux_sr, c, Cc) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  v.x = operand_op(op.op, v.x, y.x);
+  v.y = (c + 1 < Cc) ? operand_op(op.op, v.y, y.y) : 0.0f;
+  v.z = (c + 2 < Cc) ? operand_op(op.op, v.z, y.z) : 0.0f;
+  v.w = (c + 3 < Cc) ? operand_op(op.op, v.w, y.w) : 0.0f;
+  return v;
+}
+
 // src: R rows of Cc contiguous floats, leading dimension src_ld (16-byte aligned rows).
 // hi/lo: compact, leading dimension dst_ld (multiple of 4).
+template <bool HAS_OP = false>
 __global__ void __launch_bounds__(256)
 split_rows_tf32_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld,
-                       float *__restrict__ hi, float *__restrict__ lo, int64_t dst_ld) {
+                       float *__restrict__ hi, float *__restrict__ lo, int64_t dst_ld, OperandOp op = OperandOp()) {
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   const int64_t vec_per_row = (Cc + 3) >> 2;
   const int64_t total = R * vec_per_row;
@@ -65,6 +119,7 @@ split_rows_tf32_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int
       v.z = (c + 2 < Cc) ? s[2] : 0.0f;
       v.w = 0.0f;
     }
+    if constexpr (HAS_OP) v = op_vec(op, v, r, c, Cc);
     float4 h, l;
     h.x = tf32_rna(v.x); l.x = tf32_lo(v.x, h.x);
     h.y = tf32_rna(v.y); l.y = tf32_lo(v.y, h.y);
@@ -87,9 +142,11 @@ __device__ __forceinline__ uint32_t finite_abs_bits(float f) {
 }
 constexpr int ABSMAX_ROW_CHUNK = 1024;   // floats of one row reduced by one warp pass (32 lanes x 8 x float4)
 constexpr int ABSMAX_COL_ROWS = 64;      // rows of a 4-column strip reduced by one thread
-template <bool PER_COL>
+template <bool PER_COL, bool HAS_OP = false>
 __global__ void __launch_bounds__(256)
-absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld, uint32_t *__restrict__ out) {
+absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld, uint32_t *__restrict__ out,
+                 OperandOp op = OperandOp()) {
+  static_assert(PER_COL || !HAS_OP, "a K-major operand with an op takes the fused row kernel");
   if constexpr (!PER_COL) {
     // warp w takes (row, chunk) items; lanes read float4s 128 floats apart; butterfly max; one atomic per item
     const int lane = threadIdx.x & 31;
@@ -131,7 +188,11 @@ absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t s
       uint32_t m0 = 0u, m1 = 0u, m2 = 0u, m3 = 0u;
       for (int64_t r = rb * ABSMAX_COL_ROWS; r < r1; ++r) {
         const float *s = src + r * src_ld + c;
-        if (c + 4 <= Cc) {
+        if constexpr (HAS_OP) {   // the scale is taken over the op's output (padding lanes are 0)
+          const float4 v = op_vec(op, load_row_vec(src + r * src_ld, c, Cc), r, c, Cc);
+          m0 = max(m0, finite_abs_bits(v.x)); m1 = max(m1, finite_abs_bits(v.y));
+          m2 = max(m2, finite_abs_bits(v.z)); m3 = max(m3, finite_abs_bits(v.w));
+        } else if (c + 4 <= Cc) {
           const float4 v = *reinterpret_cast<const float4 *>(s);
           m0 = max(m0, finite_abs_bits(v.x)); m1 = max(m1, finite_abs_bits(v.y));
           m2 = max(m2, finite_abs_bits(v.z)); m3 = max(m3, finite_abs_bits(v.w));
@@ -149,18 +210,6 @@ absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t s
   }
 }
 
-__device__ __forceinline__ float4 load_row_vec(const float *row, int64_t c, int64_t Cc) {
-  float4 v;
-  if (c + 4 <= Cc) {
-    v = *reinterpret_cast<const float4 *>(row + c);
-  } else {   // ragged end of the row: one to three elements
-    v.x = row[c];
-    v.y = (c + 1 < Cc) ? row[c + 1] : 0.0f;
-    v.z = (c + 2 < Cc) ? row[c + 2] : 0.0f;
-    v.w = 0.0f;
-  }
-  return v;
-}
 __device__ __forceinline__ void store_f16x2_vec4(float4 v, float sx, float sy, float sz, float sw, uint16_t *hrow, uint16_t *lrow,
                                                  int64_t c) {
   uint2 h, l;
@@ -178,10 +227,10 @@ __device__ __forceinline__ void store_f16x2_vec(float4 v, float s, uint16_t *hro
 // thread; what is left of a longer row is read twice, the second time from L2), reduces the abs-max, writes the word and
 // both fp16 pieces: 4 bytes read + 4 written per element, against 8 + 4 for abs-max and split as two kernels.
 constexpr int F16ROWS_MAXV = 8;
-template <int GROUP>
+template <int GROUP, bool HAS_OP = false>
 __global__ void __launch_bounds__(256, 4)
 f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *__restrict__ hb,
-                        uint16_t *__restrict__ lb, int64_t ld_b, uint32_t *__restrict__ absmax) {
+                        uint16_t *__restrict__ lb, int64_t ld_b, uint32_t *__restrict__ absmax, OperandOp op = OperandOp()) {
   static_assert(GROUP == 32 || GROUP == 256, "a warp or the CTA per row");
   __shared__ uint32_t red[2][8];
   ptx::griddep_launch_dependents();
@@ -201,11 +250,13 @@ f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
       const int64_t idx = tid + static_cast<int64_t>(i) * GROUP;
       if (idx < nvec) {
         v[i] = load_row_vec(row, idx << 2, Cc);
+        if constexpr (HAS_OP) v[i] = op_vec(op, v[i], r, idx << 2, Cc);
         m = max(max(m, finite_abs_bits(v[i].x)), max(finite_abs_bits(v[i].y), max(finite_abs_bits(v[i].z), finite_abs_bits(v[i].w))));
       }
     }
     for (int64_t idx = tid + static_cast<int64_t>(F16ROWS_MAXV) * GROUP; idx < nvec; idx += GROUP) {
-      const float4 t = load_row_vec(row, idx << 2, Cc);
+      float4 t = load_row_vec(row, idx << 2, Cc);
+      if constexpr (HAS_OP) t = op_vec(op, t, r, idx << 2, Cc);
       m = max(max(m, finite_abs_bits(t.x)), max(finite_abs_bits(t.y), max(finite_abs_bits(t.z), finite_abs_bits(t.w))));
     }
     float mf = __uint_as_float(m);     // non-negative finite: fmaxf orders them like the integers
@@ -227,8 +278,10 @@ f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
       const int64_t idx = tid + static_cast<int64_t>(i) * GROUP;
       if (idx < nvec) store_f16x2_vec(v[i], s, hrow, lrow, idx << 2);
     }
-    for (int64_t idx = tid + static_cast<int64_t>(F16ROWS_MAXV) * GROUP; idx < nvec; idx += GROUP)
-      store_f16x2_vec(load_row_vec(row, idx << 2, Cc), s, hrow, lrow, idx << 2);
+    for (int64_t idx = tid + static_cast<int64_t>(F16ROWS_MAXV) * GROUP; idx < nvec; idx += GROUP) {
+      if constexpr (HAS_OP) store_f16x2_vec(op_vec(op, load_row_vec(row, idx << 2, Cc), r, idx << 2, Cc), s, hrow, lrow, idx << 2);
+      else store_f16x2_vec(load_row_vec(row, idx << 2, Cc), s, hrow, lrow, idx << 2);
+    }
   }
 }
 
@@ -318,11 +371,11 @@ inline bool f16x2_rows_ring_ok(const float *src, int64_t Cc, int64_t src_ld) {
 // SPLIT_ROWS rows): a thread owns 4 columns of the strip -- for PER_COL their four scales are computed once -- and walks
 // the rows of the block, adjacent threads reading adjacent float4s.
 constexpr int SPLIT_ROWS = 64;
-template <bool PER_COL>
+template <bool PER_COL, bool HAS_OP = false>
 __global__ void __launch_bounds__(256)
 split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld,
                         uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld_b,
-                        const uint32_t *__restrict__ absmax) {
+                        const uint32_t *__restrict__ absmax, OperandOp op = OperandOp()) {
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   const int tx = static_cast<int>(threadIdx.x) & 63, ty = static_cast<int>(threadIdx.x) >> 6;   // 64 float4 columns x 4 row lanes
   const int64_t strips = (Cc + 255) >> 8;
@@ -341,7 +394,8 @@ split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
     const int64_t r1 = (rb + 1) * SPLIT_ROWS < R ? (rb + 1) * SPLIT_ROWS : R;
 #pragma unroll 4
     for (int64_t r = rb * SPLIT_ROWS + ty; r < r1; r += 4) {
-      const float4 v = load_row_vec(src + r * src_ld, c, Cc);
+      float4 v = load_row_vec(src + r * src_ld, c, Cc);
+      if constexpr (HAS_OP) v = op_vec(op, v, r, c, Cc);
       if constexpr (!PER_COL) sx = sy = sz = sw = f16x2_scale(absmax[r]);
       store_f16x2_vec4(v, sx, sy, sz, sw, hb + r * ld_b, lb + r * ld_b, c);
     }
@@ -352,10 +406,12 @@ split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
 // memory so that both the gather (along whichever source stride is smaller) and the
 // store (along c) are coalesced.  SPLIT: also write lo (fp32 only).
 // MODE 0: plain copy; 1: fp32 hi/lo pieces (dst, dst_lo).
-template <typename T, int MODE>
+// HAS_OP (fp32): the op is applied to each element as it is gathered (aux read with its own strides).
+template <typename T, int MODE, bool HAS_OP = false>
 __global__ void __launch_bounds__(256)
 pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr, int64_t sc,
-                    T *__restrict__ dst, T *__restrict__ dst_lo, int64_t ld, int read_along_r) {
+                    T *__restrict__ dst, T *__restrict__ dst_lo, int64_t ld, int read_along_r, OperandOp op = OperandOp()) {
+  static_assert(!HAS_OP || sizeof(T) == 4, "operand ops are fp32 only");
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   __shared__ T tile[32][33];
   const int64_t tiles_c = (Cc + 31) >> 5;
@@ -367,13 +423,23 @@ pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int64_t c = c0 + ty + i * 8, r = r0 + tx;
-        if (r < R && c < Cc) tile[tx][ty + i * 8] = src[r * sr + c * sc];
+        if constexpr (HAS_OP) {
+          if (r < R && c < Cc)
+            tile[tx][ty + i * 8] = operand_op(op.op, src[r * sr + c * sc], op.aux ? op.aux[r * op.aux_sr + c * op.aux_sc] : 0.0f);
+        } else {
+          if (r < R && c < Cc) tile[tx][ty + i * 8] = src[r * sr + c * sc];
+        }
       }
     } else {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int64_t r = r0 + ty + i * 8, c = c0 + tx;
-        if (r < R && c < Cc) tile[ty + i * 8][tx] = src[r * sr + c * sc];
+        if constexpr (HAS_OP) {
+          if (r < R && c < Cc)
+            tile[ty + i * 8][tx] = operand_op(op.op, src[r * sr + c * sc], op.aux ? op.aux[r * op.aux_sr + c * op.aux_sc] : 0.0f);
+        } else {
+          if (r < R && c < Cc) tile[ty + i * 8][tx] = src[r * sr + c * sc];
+        }
       }
     }
     __syncthreads();

@@ -137,11 +137,35 @@ def gemm_strided(M, N, K, alpha, A, rowStrideA, colStrideA, B, rowStrideB, colSt
         check(getattr(L, "laser_b200_gemm_strided_%s_dev" % ta)(*args, stream))
 
 
+def _operand_op(spec):
+    """op_a / op_b of gemm_strided_fused -> an OperandOp, or None"""
+    if spec is None:
+        return None
+    if isinstance(spec, str):
+        spec = (spec,)
+    name, rest = spec[0], tuple(spec[1:])
+    op = _capi.OperandOp()
+    op.op = _capi.OP_NAMES[name]
+    if rest:
+        if len(rest) != 3:
+            raise ValueError("an operand op is a name or (name, aux, auxRowStride, auxColStride)")
+        paux, taux, daux = _resolve(rest[0])
+        if not daux or taux != "f32":
+            raise TypeError("aux must be a float32 device buffer")
+        op.aux = paux
+        op.auxRowStride, op.auxColStride = int(rest[1]), int(rest[2])
+    return op
+
+
 def gemm_strided_fused(M, N, K, alpha, A, rowStrideA, colStrideA, B, rowStrideB, colStrideB, beta, C,
                        rowStrideC, colStrideC, bias=None, bias_per_row=False, activation="none",
-                       path=PATH_AUTO, stream=None):
-    """C <- act(alpha*A*B + beta*C + bias) on float32 DEVICE buffers: the epilogue fusion the
-    reference lists as its next step (gemm.nim:196).  activation: none | relu | tanh | sigmoid."""
+                       path=PATH_AUTO, stream=None, *, op_a=None, op_b=None):
+    """C <- act(alpha*opA(A)*opB(B) + beta*C + bias) on float32 DEVICE buffers: the epilogue fusion the
+    reference lists as its next step (gemm.nim:196).  activation: none | relu | tanh | sigmoid.
+    op_a / op_b (the prologue fusion): an elementwise op applied to the operand while it is prepared --
+    "relu", "tanh", "sigmoid", or a derivative with its aux tensor and that tensor's element strides,
+    e.g. op_a=("relu_grad", Z, rowStrideZ, colStrideZ) for dY * relu'(Z); also "tanh_grad" (aux: the
+    tanh output) and "sigmoid_grad" (aux: the sigmoid output)."""
     pa, ta, da = _resolve(A); pb, tb, db = _resolve(B); pc, tc, dc = _resolve(C)
     if not (ta == tb == tc == "f32") or not (da and db and dc):
         raise TypeError("gemm_strided_fused takes float32 device buffers")
@@ -153,11 +177,19 @@ def gemm_strided_fused(M, N, K, alpha, A, rowStrideA, colStrideA, B, rowStrideB,
         epi.bias = pbias
     epi.bias_per_row = 1 if bias_per_row else 0
     epi.activation = {"none": 0, "relu": 1, "tanh": 2, "sigmoid": 3}[activation]
+    oa, ob = _operand_op(op_a), _operand_op(op_b)
     if stream is None:
         stream = _current_stream()
-    check(lib().laser_b200_gemm_strided_f32_epi_dev(M, N, K, float(alpha), pa, rowStrideA, colStrideA, pb, rowStrideB,
-                                                    colStrideB, float(beta), pc, rowStrideC, colStrideC,
-                                                    ctypes.byref(epi), path, stream))
+    if oa is None and ob is None:
+        check(lib().laser_b200_gemm_strided_f32_epi_dev(M, N, K, float(alpha), pa, rowStrideA, colStrideA, pb, rowStrideB,
+                                                        colStrideB, float(beta), pc, rowStrideC, colStrideC,
+                                                        ctypes.byref(epi), path, stream))
+        return
+    check(lib().laser_b200_gemm_strided_f32_fused_dev(M, N, K, float(alpha), pa, rowStrideA, colStrideA, pb, rowStrideB,
+                                                      colStrideB, float(beta), pc, rowStrideC, colStrideC,
+                                                      ctypes.byref(oa) if oa is not None else None,
+                                                      ctypes.byref(ob) if ob is not None else None,
+                                                      ctypes.byref(epi), path, stream))
 
 
 def last_path():

@@ -22,6 +22,19 @@ type
   GemmPath* {.size: sizeof(cint).} = enum      # LASER_B200_PATH_*
     pathAuto = 0, pathSimt = 1, pathTf32x1 = 2, pathTf32x3 = 3, pathBf16 = 4, pathF16x3 = 7   # 7: the default fp32 mode
 
+  LaserB200Epilogue* {.bycopy.} = object       # laser_b200_epilogue
+    bias*: ptr float32
+    bias_per_row*: int32
+    activation*: int32                         # LASER_B200_ACT_*: 0 none, 1 relu, 2 tanh, 3 sigmoid
+
+  OperandOpKind* {.size: sizeof(int32).} = enum  # LASER_B200_OP_*
+    opNone = 0, opRelu = 1, opTanh = 2, opSigmoid = 3, opReluGrad = 4, opTanhGrad = 5, opSigmoidGrad = 6
+
+  LaserB200OperandOp* {.bycopy.} = object      # laser_b200_operand_op: the fused prologue (README.md:244-245)
+    op*: OperandOpKind
+    aux*: ptr float32                          # device; the derivative ops only
+    auxRowStride*, auxColStride*: int64
+
 {.push importc, cdecl, dynlib: laserB200Lib.}
 proc laser_b200_init*(): cint
 proc laser_b200_shutdown*()
@@ -86,6 +99,17 @@ proc laser_b200_gemm_packed_f32_dev*(M, N, K: int64, alpha: float32, packedA, pa
 proc laser_b200_gemm_packedB_f32_dev*(M, N, K: int64, alpha: float32, A: ptr float32,
     rowStrideA, colStrideA: int64, packedB: pointer, beta: float32, C: ptr float32,
     rowStrideC, colStrideC: int64, stream: pointer): cint
+proc laser_b200_gemm_strided_f32_epi_dev*(M, N, K: int64, alpha: float32,
+    A: ptr float32, rowStrideA, colStrideA: int64,
+    B: ptr float32, rowStrideB, colStrideB: int64,
+    beta: float32, C: ptr float32, rowStrideC, colStrideC: int64,
+    epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
+# fused prologue: C <- act(alpha * opA(A) * opB(B) + beta * C + bias) (README.md:244-245); nil = no op
+proc laser_b200_gemm_strided_f32_fused_dev*(M, N, K: int64, alpha: float32,
+    A: ptr float32, rowStrideA, colStrideA: int64,
+    B: ptr float32, rowStrideB, colStrideB: int64,
+    beta: float32, C: ptr float32, rowStrideC, colStrideC: int64,
+    opA, opB: ptr LaserB200OperandOp, epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
 proc laser_b200_malloc*(devPtr: ptr pointer, bytes: csize_t): cint
 proc laser_b200_free*(devPtr: pointer): cint
 proc laser_b200_memcpy_h2d*(dst, src: pointer, bytes: csize_t): cint
