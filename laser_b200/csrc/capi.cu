@@ -101,7 +101,6 @@ struct Ctx {
   int raster_g = 0;       // env LASER_B200_RASTER (0 = default)
   bool splitk_enabled = true;  // env LASER_B200_SPLITK=0 disables split-K
   bool f64_dmma = true;        // env LASER_B200_F64_DMMA=0: fp64 problems stay on the CUDA-core kernel
-  bool prep_ring = true;       // env LASER_B200_PREP_RING=0: register-only preparation kernel for K-major operands
   bool ring_attr_set = false, dmma_attr_set = false;
   int64_t panel_rows = 1024;  // env LASER_B200_PANEL_ROWS: row-panel height of the pipelined host-pointer entry
   bool panel_taper = false;   // env LASER_B200_PANEL_TAPER=1: cut the last row panel finer (shorter PCIe tail)
@@ -192,7 +191,6 @@ int get_ctx(Ctx **out) {
       if (const char *cp = getenv("LASER_B200_CTA_PAIR")) c.cta_pair = atoi(cp) != 0;
       if (const char *rg = getenv("LASER_B200_RASTER")) c.raster_g = atoi(rg);
       if (const char *sk = getenv("LASER_B200_SPLITK")) c.splitk_enabled = atoi(sk) != 0;
-      if (const char *pr = getenv("LASER_B200_PREP_RING")) c.prep_ring = atoi(pr) != 0;
       if (const char *dm = getenv("LASER_B200_F64_DMMA")) c.f64_dmma = atoi(dm) != 0;
       if (const char *pt = getenv("LASER_B200_PANEL_TAPER")) c.panel_taper = atoi(pt) != 0;
       if (const char *ds = getenv("LASER_B200_DYNSCHED")) c.dyn_sched = atoi(ds) != 0;
@@ -221,28 +219,41 @@ int ensure(Buffer &b, size_t bytes) {
   return LASER_B200_OK;
 }
 
-int prof_open(Ctx &c, cudaStream_t s, EventPair *ep, int kind) {
-  if (!c.profiling) return LASER_B200_OK;
-  ep->kind = kind;
-  ep->launches = 0;
-  CUDA_TRY(cudaEventCreate(&ep->a));
-  CUDA_TRY(cudaEventCreate(&ep->b));
-  CUDA_TRY(cudaEventRecord(ep->a, s));
-  return LASER_B200_OK;
-}
-int prof_close(Ctx &c, cudaStream_t s, EventPair *ep, int launches) {
-  if (!c.profiling) return LASER_B200_OK;
-  CUDA_TRY(cudaEventRecord(ep->b, s));
-  ep->launches = launches;
-  c.prof.push_back(*ep);
-  return LASER_B200_OK;
-}
+// Profiling bracket around a group of launches on one stream.  launches(): how many were made since open(), counted
+// whether profiling is on or not.  With profiling on, close() records the pair with that count; a bracket that is left
+// without close() (an error return) releases its events unrecorded.
+struct ProfBracket {
+  Ctx *c = nullptr;   // set while events are held
+  cudaStream_t s = nullptr;
+  EventPair ep{};
+  int64_t before = 0;
 
-void prof_abort(Ctx &c, EventPair *ep) {   // an error path after prof_open: the pair is not recorded, so release it here
-  if (!c.profiling) return;
-  cudaEventDestroy(ep->a);
-  cudaEventDestroy(ep->b);
-}
+  int open(Ctx &ctx, cudaStream_t stream, int kind) {
+    before = g_launches.load();
+    if (!ctx.profiling) return LASER_B200_OK;
+    c = &ctx;
+    s = stream;
+    ep.kind = kind;
+    CUDA_TRY(cudaEventCreate(&ep.a));
+    CUDA_TRY(cudaEventCreate(&ep.b));
+    CUDA_TRY(cudaEventRecord(ep.a, s));
+    return LASER_B200_OK;
+  }
+  int launches() const { return static_cast<int>(g_launches.load() - before); }
+  int close() {
+    if (!c) return LASER_B200_OK;
+    ep.launches = launches();
+    CUDA_TRY(cudaEventRecord(ep.b, s));
+    c->prof.push_back(ep);
+    c = nullptr;
+    return LASER_B200_OK;
+  }
+  ~ProfBracket() {
+    if (!c) return;
+    if (ep.a) cudaEventDestroy(ep.a);
+    if (ep.b) cudaEventDestroy(ep.b);
+  }
+};
 
 inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 inline int grid_for(const Ctx &c, int64_t work_items, int per_sm) {
@@ -428,79 +439,6 @@ enum SplitMode {
   SPLIT_F16X2 = 2,   // abs-max word per mn index + two fp16 pieces of the scaled operand (F16X3, the default)
 };
 
-// F16X3 preparation of a row-contiguous fp32 operand [R][Cc] (mn along R, or along Cc when the operand is MN-major):
-// K-major: ONE fused pass (abs-max per row, scale, split; split.cuh).  MN-major: the scale belongs to a column, so the
-// abs-max pass (strip reduction + atomicMax) comes first and the split second.  HAS_OP: both passes apply `op` on load, so
-// the scale words are those of the op's output.  The ring kernel has no op variant: long op'd rows take the register kernel.
-template <bool HAS_OP>
-int f16x2_prepare(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, bool mn_along_cols, const OperandWs &w,
-                  int64_t ld_b, cudaStream_t s, const OperandOp &op) {
-  uint32_t *words = static_cast<uint32_t *>(c.f16s.ptr) + w.amax_off;
-  const int64_t n_mn = mn_along_cols ? Cc : R;
-  if (c.f16s.bytes < static_cast<size_t>(w.amax_off + n_mn) * sizeof(uint32_t))
-    return set_error(LASER_B200_ECUDA, "internal: F16X3 scale buffer not sized for this operand");
-  uint16_t *xb = static_cast<uint16_t *>(w.p0->ptr), *lb = static_cast<uint16_t *>(w.p1->ptr);
-  if (mn_along_cols) {
-    CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(n_mn) * sizeof(uint32_t), s));
-    const int64_t items = ((Cc + 3) / 4) * ((R + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS);
-    absmax_mn_kernel<true, HAS_OP><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(src, R, Cc, src_ld, words, op);
-    COUNT_LAUNCH();
-    CHECK_LAUNCH();
-    const int64_t split_items = ((Cc + 255) / 256) * ((R + SPLIT_ROWS - 1) / SPLIT_ROWS);
-    split_rows_f16x2_kernel<true, HAS_OP><<<grid_for(c, split_items, 8), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words, op);
-  } else if (Cc <= 4 * 32 * F16ROWS_MAXV) {   // short rows: a warp per row
-    f16x2_rows_fused_kernel<32, HAS_OP><<<grid_for(c, (R + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words, op);
-  } else if (!HAS_OP && c.prep_ring && f16x2_rows_ring_ok(src, Cc, src_ld)) {   // rows prefetched into a shared-memory ring by the copy engine
-    const size_t smem = f16x2_rows_ring_smem(Cc);
-    if (!c.ring_attr_set) {
-      CUDA_TRY(cudaFuncSetAttribute(f16x2_rows_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    static_cast<int>(f16x2_rows_ring_smem(4 * 256 * F16ROWS_MAXV))));
-      c.ring_attr_set = true;
-    }
-    f16x2_rows_ring_kernel<<<grid_for(c, R, 2), 256, smem, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words);
-  } else {
-    f16x2_rows_fused_kernel<256, HAS_OP><<<grid_for(c, R, 4), 256, 0, s>>>(src, R, Cc, src_ld, xb, lb, ld_b, words, op);
-  }
-  COUNT_LAUNCH();
-  CHECK_LAUNCH();
-  return LASER_B200_OK;
-}
-
-// capi_multi.inc (rowshard_prepared): the root prepares B panel by panel into a panel-major buffer.
-// Scale words of every column of a row-major B [K][N] (a column's scale needs the whole column):
-int f16x2_absmax_cols(Ctx &c, const float *B, int64_t K, int64_t N, int64_t ld, uint32_t *words, cudaStream_t s) {
-  CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(N) * sizeof(uint32_t), s));
-  const int64_t items = ((N + 3) / 4) * ((K + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS);
-  absmax_mn_kernel<true><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(B, K, N, ld, words, OperandOp());
-  COUNT_LAUNCH();
-  CHECK_LAUNCH();
-  return LASER_B200_OK;
-}
-// One column panel (w columns) of B into its two fp16 pieces.  Row-major B: Bp = first column of the panel, ld = row
-// pitch, pieces [K][w] (MN-major), `words` already hold the panel's scales.  Column-major B: Bp = first column (a contiguous
-// row of K floats), ld = column pitch, pieces [w][K] (K-major), scale words written in the same pass.
-int f16x2_prepare_panel(Ctx &c, bool row_major, const float *Bp, int64_t K, int64_t w, int64_t ld, uint16_t *hi, uint16_t *lo,
-                        uint32_t *words, cudaStream_t s) {
-  if (row_major) {
-    const int64_t split_items = ((w + 255) / 256) * ((K + SPLIT_ROWS - 1) / SPLIT_ROWS);
-    split_rows_f16x2_kernel<true><<<grid_for(c, split_items, 8), 256, 0, s>>>(Bp, K, w, ld, hi, lo, w, words, OperandOp());
-  } else if (K <= 4 * 32 * F16ROWS_MAXV) {
-    f16x2_rows_fused_kernel<32><<<grid_for(c, (w + 7) / 8, 4), 256, 0, s>>>(Bp, w, K, ld, hi, lo, K, words, OperandOp());
-  } else if (c.prep_ring && f16x2_rows_ring_ok(Bp, K, ld)) {
-    if (!c.ring_attr_set) {
-      CUDA_TRY(cudaFuncSetAttribute(f16x2_rows_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    static_cast<int>(f16x2_rows_ring_smem(4 * 256 * F16ROWS_MAXV))));
-      c.ring_attr_set = true;
-    }
-    f16x2_rows_ring_kernel<<<grid_for(c, w, 2), 256, f16x2_rows_ring_smem(K), s>>>(Bp, w, K, ld, hi, lo, K, words);
-  } else {
-    f16x2_rows_fused_kernel<256><<<grid_for(c, w, 4), 256, 0, s>>>(Bp, w, K, ld, hi, lo, K, words, OperandOp());
-  }
-  COUNT_LAUNCH();
-  CHECK_LAUNCH();
-  return LASER_B200_OK;
-}
-
 // Operand ops of the fused-prologue entry.  Host side, `OperandOp` describes aux as [mn][k] like its Operand
 // (aux_sr = s_mn, aux_sc = s_k); the preparation kernels see it over their [R][Cc] rows, where R runs along k when the
 // prepared layout is MN-major.
@@ -513,121 +451,156 @@ inline OperandOp kernel_op(const OperandOp &op, bool rows_along_k) {
 inline bool op_same_layout(const Operand &o, const OperandOp &op) {
   return !op.aux || (op.aux_sr == o.s_mn && op.aux_sc == o.s_k && (reinterpret_cast<uintptr_t>(op.aux) & 15) == 0);
 }
-// op(operand) gathered into a compact fp32 [mn][round_up(k, 4)] array (aux read with its own strides)
-int gather_op(Ctx &c, const Operand &o, const OperandOp &op, Buffer &dst, cudaStream_t s, const float **out) {
-  const int64_t ld = round_up(o.k, 4);
-  int rc;
-  if ((rc = ensure(dst, static_cast<size_t>(o.mn) * ld * sizeof(float)))) return rc;
-  const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32);
-  const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
-  pack_general_kernel<float, 0, true><<<grid_for(c, tiles, 8), 256, 0, s>>>(static_cast<const float *>(o.ptr), o.mn, o.k, o.s_mn,
-                                                                           o.s_k, static_cast<float *>(dst.ptr), nullptr, ld,
-                                                                           read_along_r, op);
+
+// ---- the preparation steps: one function, and one launch site, per kernel family of split.cuh ----
+// A step takes its op as a pointer (nullptr: none) and hands `launch` either (std::true_type, *op) or
+// (std::false_type, OperandOp()): the kernel's HAS_OP and plain instantiations come from the same launch statement.
+template <typename Launch>
+int launch_prep(const OperandOp *op, Launch launch) {
+  if (op) launch(std::true_type(), *op);
+  else launch(std::false_type(), OperandOp());
   COUNT_LAUNCH();
   CHECK_LAUNCH();
-  *out = static_cast<const float *>(dst.ptr);
   return LASER_B200_OK;
 }
 
-// op: nullptr, or an operand op (fp32 operands only)
+// The gather: op(operand), or the operand itself, from any strides into compact K-major rows [mn][round_up(k, 16 / sizeof(T))]
+// allocated in dst (aux read with its own strides).  MODE 1 (fp32): the tf32 hi / lo pieces into dst / *lo.  bf16 operands
+// carry no op.
+template <typename T, int MODE = 0>
+int gather(Ctx &c, const Operand &o, Buffer &dst, Buffer *lo, cudaStream_t s, const OperandOp *op = nullptr) {
+  const int64_t ld = round_up(o.k, 16 / static_cast<int64_t>(sizeof(T)));
+  const size_t bytes = static_cast<size_t>(o.mn) * ld * sizeof(T);
+  int rc;
+  if ((rc = ensure(dst, bytes))) return rc;
+  if (MODE == 1 && (rc = ensure(*lo, bytes))) return rc;
+  const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32);
+  const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
+  T *d0 = static_cast<T *>(dst.ptr), *d1 = MODE == 1 ? static_cast<T *>(lo->ptr) : nullptr;
+  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
+    pack_general_kernel<T, MODE, decltype(has_op)::value && sizeof(T) == 4><<<grid_for(c, tiles, 8), 256, 0, s>>>(
+        static_cast<const T *>(o.ptr), o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, k);
+  });
+}
+
+// TF32X3 in place: tf32 hi / lo pieces [R][ld] of fp32 rows [R][Cc], src_ld apart
+int tf32_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, float *hi, float *lo, int64_t ld, cudaStream_t s,
+               const OperandOp *op) {
+  const int64_t items = R * ((Cc + 3) / 4);
+  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
+    split_rows_tf32_kernel<decltype(has_op)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
+        src, R, Cc, src_ld, hi, lo, ld, k);
+  });
+}
+
+// F16X3, one scale per row of fp32 rows [R][Cc] (src_ld apart): the abs-max word of each row, the scale and the two fp16
+// pieces [R][ld_b] in ONE pass (split.cuh).  Rows of up to 1024 floats: a warp per row.  Longer rows: prefetched into a
+// shared-memory ring by the copy engine when they allow it (16-byte aligned, at most 8192 floats; the ring kernel has no op
+// variant), the CTA per row otherwise.
+int f16x2_rows(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *hb, uint16_t *lb, int64_t ld_b,
+               uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
+  const bool ring = !op && f16x2_rows_ring_ok(src, Cc, src_ld);
+  if (ring && !c.ring_attr_set) {
+    CUDA_TRY(cudaFuncSetAttribute(f16x2_rows_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(f16x2_rows_ring_smem(4 * 256 * F16ROWS_MAXV))));
+    c.ring_attr_set = true;
+  }
+  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
+    constexpr bool HAS_OP = decltype(has_op)::value;
+    if (Cc <= 4 * 32 * F16ROWS_MAXV)
+      f16x2_rows_fused_kernel<32, HAS_OP><<<grid_for(c, (R + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words, k);
+    else if (ring)
+      f16x2_rows_ring_kernel<<<grid_for(c, R, 2), 256, f16x2_rows_ring_smem(Cc), s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words);
+    else
+      f16x2_rows_fused_kernel<256, HAS_OP><<<grid_for(c, R, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words, k);
+  });
+}
+
+// F16X3, one scale per column of fp32 rows [R][Cc]: the abs-max word of every column (zeroed here, then strip reductions
+// combined by atomicMax).  A column's scale needs the whole column, so the split is a second pass.
+int f16x2_col_scales(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint32_t *words, cudaStream_t s,
+                     const OperandOp *op = nullptr) {
+  CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(Cc) * sizeof(uint32_t), s));
+  const int64_t items = ((Cc + 3) / 4) * ((R + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS);
+  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
+    absmax_mn_kernel<true, decltype(has_op)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
+        src, R, Cc, src_ld, words, k);
+  });
+}
+// F16X3, one scale per column: the two fp16 pieces [R][ld_b] of fp32 rows [R][Cc] against the columns' scale words
+int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *hb, uint16_t *lb, int64_t ld_b,
+                    const uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
+  const int64_t items = ((Cc + 255) / 256) * ((R + SPLIT_ROWS - 1) / SPLIT_ROWS);
+  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
+    split_rows_f16x2_kernel<true, decltype(has_op)::value><<<grid_for(c, items, 8), 256, 0, s>>>(
+        src, R, Cc, src_ld, hb, lb, ld_b, words, k);
+  });
+}
+
+// One operand of a tensor-core call: first the plan, then its steps.
+//   bf16 K- or MN-major; TF32X1 K-major without op: TMA reads the caller's memory, no workspace.
+//   TF32X3 K-major; F16X3 K- or MN-major -- without op, or with aux laid out like the operand: the split reads the caller's
+//     memory and applies the op on load (F16X3 MN-major: all column scales first, then the split).
+//   Anything else: one gather, which applies the op, into compact K-major rows.  TMA reads those (bf16, TF32X1), the gather
+//     splits them on the way (TF32X3), or the plain row kernel prepares them (F16X3).
+// wgmma reads tf32 tiles K-major only, and TMA applies no op.  op: nullptr, or an operand op (fp32 operands only).
 template <int ESZ>
 int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w, int block_mn,
                     OperandMaps *m, bool *used_ws, cudaStream_t s, const OperandOp *op = nullptr) {
-  using ET = typename std::conditional<ESZ == 4, float, uint16_t>::type;
-  // wgmma reads tf32 tiles K-major only: an MN-major fp32 operand of the tf32 modes is gathered into compact K-major rows
-  const Major mj0 = classify(o, ESZ);
-  Major mj = (ESZ == 4 && mode != SPLIT_F16X2 && mj0 == MN_MAJOR) ? GENERAL : mj0;
-  // an op is applied on load by the preparation kernels when aux has the operand's layout; otherwise, and when TMA would
-  // read the caller's memory as it is (SPLIT_NONE), one gather applies it
-  if (op && mj != GENERAL && (mode == SPLIT_NONE || !op_same_layout(o, *op))) mj = GENERAL;
-  const int64_t vec = 16 / ESZ;
+  const Major mj = classify(o, ESZ);
+  const bool tma_layout = mj == K_MAJOR || (mj == MN_MAJOR && (ESZ == 2 || mode == SPLIT_F16X2));
+  const bool in_place = tma_layout && (!op || (mode != SPLIT_NONE && op_same_layout(o, *op)));
+  const Major out_mj = in_place ? mj : K_MAJOR;              // layout of the arrays the tensor-core kernel reads
+  const int64_t R = (out_mj == K_MAJOR) ? o.mn : o.k;        // their rows
+  const int64_t Cc = (out_mj == K_MAJOR) ? o.k : o.mn;       // their contiguous extent
+  const int64_t src_ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;   // row pitch of the operand, read in place
+  const int64_t ld = round_up(Cc, 16 / ESZ);
+  m->mn_major = (out_mj == MN_MAJOR);
   int rc;
-  if (mj != GENERAL && mode == SPLIT_NONE) {
-    const int64_t ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;
-    m->mn_major = (mj == MN_MAJOR);
-    if ((rc = operand_map(c, &m->p0, ESZ, o.ptr, mj, o.mn, o.k, ld, block_mn))) return rc;
+  if (mode == SPLIT_NONE && in_place) {
+    if ((rc = operand_map(c, &m->p0, ESZ, o.ptr, mj, o.mn, o.k, src_ld, block_mn))) return rc;
     m->p1 = m->p0;
     return LASER_B200_OK;
   }
   *used_ws = true;
-  // layout of the prepared arrays: the operand's own major-ness when TMA can address it,
-  // compact K-major [mn][k] after a gather otherwise
-  const Major out_mj = (mj == GENERAL) ? K_MAJOR : mj;
-  const int64_t R = (out_mj == K_MAJOR) ? o.mn : o.k;    // rows of the prepared arrays
-  const int64_t Cc = (out_mj == K_MAJOR) ? o.k : o.mn;   // contiguous extent
-  const int64_t ld = round_up(Cc, vec);
-  const int64_t ld_b = round_up(Cc, 8);
-  const size_t bytes = static_cast<size_t>(R) * ld * ESZ;
-  const size_t bytes_b = static_cast<size_t>(R) * ld_b * 2;
-  m->mn_major = (out_mj == MN_MAJOR);
-  if constexpr (ESZ == 4) {
+  if constexpr (ESZ == 2) {
+    if ((rc = gather<uint16_t>(c, o, *w.p0, nullptr, s))) return rc;
+  } else {
+    const float *src = static_cast<const float *>(o.ptr);
+    const OperandOp kop = op ? kernel_op(*op, out_mj == MN_MAJOR) : OperandOp();
+    const OperandOp *on_load = (in_place && op) ? &kop : nullptr;
     if (mode == SPLIT_F16X2) {
+      const int64_t ld_b = round_up(Cc, 8);
+      const size_t bytes_b = static_cast<size_t>(R) * ld_b * 2;
       if ((rc = ensure(*w.p0, bytes_b))) return rc;
       if ((rc = ensure(*w.p1, bytes_b))) return rc;
-      const float *src = static_cast<const float *>(o.ptr);
-      int64_t src_ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;
-      if (mj == GENERAL && op) {   // the op applied by the gather; what follows is the plain preparation of its output
-        if ((rc = gather_op(c, o, *op, *w.gather, s, &src))) return rc;
-        src_ld = ld;
-      } else if (mj == GENERAL) {
-        // general strides: one coalesced gather into a compact fp32 array (the surviving descendant of pack_A / pack_B),
-        // then the fused scale + split of that
-        if ((rc = ensure(*w.gather, bytes))) return rc;
-        const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32);
-        const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
-        pack_general_kernel<float, 0><<<grid_for(c, tiles, 8), 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k,
-                                                                            static_cast<float *>(w.gather->ptr), nullptr, ld,
-                                                                            read_along_r, OperandOp());
-        COUNT_LAUNCH();
-        CHECK_LAUNCH();
-        src = static_cast<const float *>(w.gather->ptr);
-        src_ld = ld;
+      if (c.f16s.bytes < static_cast<size_t>(w.amax_off + o.mn) * sizeof(uint32_t))
+        return set_error(LASER_B200_ECUDA, "internal: F16X3 scale buffer not sized for this operand");
+      uint16_t *hb = static_cast<uint16_t *>(w.p0->ptr), *lb = static_cast<uint16_t *>(w.p1->ptr);
+      uint32_t *words = static_cast<uint32_t *>(c.f16s.ptr) + w.amax_off;
+      if (!in_place) {
+        if ((rc = gather<float>(c, o, *w.gather, nullptr, s, op))) return rc;
+        rc = f16x2_rows(c, static_cast<const float *>(w.gather->ptr), R, Cc, ld, hb, lb, ld_b, words, s);
+      } else if (out_mj == K_MAJOR) {
+        rc = f16x2_rows(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load);
+      } else {
+        if ((rc = f16x2_col_scales(c, src, R, Cc, src_ld, words, s, on_load))) return rc;
+        rc = f16x2_col_split(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load);
       }
-      rc = (op && mj != GENERAL)
-               ? f16x2_prepare<true>(c, src, R, Cc, src_ld, out_mj == MN_MAJOR, w, ld_b, s, kernel_op(*op, out_mj == MN_MAJOR))
-               : f16x2_prepare<false>(c, src, R, Cc, src_ld, out_mj == MN_MAJOR, w, ld_b, s, OperandOp());
       if (rc) return rc;
       if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, o.k, ld_b, block_mn))) return rc;
       return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, o.k, ld_b, block_mn);
     }
-  }
-  if ((rc = ensure(*w.p0, bytes))) return rc;
-  if (mode == SPLIT_TF32 && (rc = ensure(*w.p1, bytes))) return rc;
-  if (mj != GENERAL) {
-    // TMA-addressable: elementwise split that keeps the operand's major-ness (fp32 only; SPLIT_NONE returned above)
-    if constexpr (ESZ == 4) {
-      const int64_t src_ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;
-      const int64_t items = R * ((Cc + 3) / 4);
-      float *hi = static_cast<float *>(w.p0->ptr), *lo = static_cast<float *>(w.p1->ptr);
-      if (op)
-        split_rows_tf32_kernel<true><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
-            static_cast<const float *>(o.ptr), R, Cc, src_ld, hi, lo, ld, kernel_op(*op, mj == MN_MAJOR));
-      else
-        split_rows_tf32_kernel<false><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
-            static_cast<const float *>(o.ptr), R, Cc, src_ld, hi, lo, ld, OperandOp());
+    if (!in_place) {
+      rc = (mode == SPLIT_TF32) ? gather<float, 1>(c, o, *w.p0, w.p1, s, op) : gather<float>(c, o, *w.p0, nullptr, s, op);
+    } else {   // TF32X3, K-major
+      const size_t bytes = static_cast<size_t>(R) * ld * sizeof(float);
+      if ((rc = ensure(*w.p0, bytes))) return rc;
+      if ((rc = ensure(*w.p1, bytes))) return rc;
+      rc = tf32_split(c, src, R, Cc, src_ld, static_cast<float *>(w.p0->ptr), static_cast<float *>(w.p1->ptr), ld, s, on_load);
     }
-  } else {
-    const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32);
-    const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
-    const int grid = grid_for(c, tiles, 8);
-    const ET *src = static_cast<const ET *>(o.ptr);
-    ET *d0 = static_cast<ET *>(w.p0->ptr);
-    if constexpr (ESZ == 4) {
-      float *d1 = static_cast<float *>(w.p1->ptr);
-      if (mode == SPLIT_TF32 && op)
-        pack_general_kernel<float, 1, true><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, *op);
-      else if (mode == SPLIT_TF32)
-        pack_general_kernel<float, 1><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, OperandOp());
-      else if (op)
-        pack_general_kernel<float, 0, true><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r, *op);
-      else
-        pack_general_kernel<float, 0><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r, OperandOp());
-    } else {
-      pack_general_kernel<ET, 0><<<grid, 256, 0, s>>>(src, o.mn, o.k, o.s_mn, o.s_k, d0, nullptr, ld, read_along_r, OperandOp());
-    }
+    if (rc) return rc;
   }
-  COUNT_LAUNCH();
-  CHECK_LAUNCH();
   if ((rc = operand_map(c, &m->p0, ESZ, w.p0->ptr, out_mj, o.mn, o.k, ld, block_mn))) return rc;
   m->p1 = m->p0;
   if (mode == SPLIT_TF32) return operand_map(c, &m->p1, ESZ, w.p1->ptr, out_mj, o.mn, o.k, ld, block_mn);
@@ -692,17 +665,17 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
     CHECK_LAUNCH();
     return LASER_B200_OK;
   };
-  EventPair ep;
-  int rc = prof_open(c, s, &ep, 0);
+  ProfBracket prof;
+  int rc = prof.open(c, s, 0);
   if (rc) return rc;
   if (p.k_splits > 1) {
     if constexpr (std::is_same<OutT, float>::value) {
       // units past the direct tiles write raw partial sums to tile-local planes of the workspace (tc_params.h); a second
       // kernel adds the planes of those tiles and applies alpha / beta / epilogue
       const int64_t ws_floats = tc_split_ws_floats(p, pair);
-      if ((rc = ensure(c.splitk, static_cast<size_t>(ws_floats) * sizeof(float)))) { prof_abort(c, &ep); return rc; }
+      if ((rc = ensure(c.splitk, static_cast<size_t>(ws_floats) * sizeof(float)))) return rc;
       p.split_ws = static_cast<float *>(c.splitk.ptr);
-      if ((rc = launch(l))) { prof_abort(c, &ep); return rc; }
+      if ((rc = launch(l))) return rc;
       const int n_tail = p.num_m_blocks * p.num_n_blocks - p.n_direct;
       const int tile_m = pair ? 2 * TC_BLOCK_M : TC_BLOCK_M;
       const int64_t items = (static_cast<int64_t>(n_tail) * tile_m * (TC_BLOCK_N / 4) + 255) / 256;
@@ -712,11 +685,11 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
       COUNT_LAUNCH();
       CHECK_LAUNCH();
       CUDA_TRY(cudaEventRecord(c.ws_free, s));  // the planes are workspace too
-      return prof_close(c, s, &ep, 2);
+      return prof.close();
     }
   }
-  if ((rc = launch(l))) { prof_abort(c, &ep); return rc; }
-  return prof_close(c, s, &ep, 1);
+  if ((rc = launch(l))) return rc;
+  return prof.close();
 }
 
 // SRC_ESZ: element size of the caller's operands (4: fp32 in any of the three tensor-core modes, 2: bf16)
@@ -738,22 +711,18 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   bool used_ws = false;
   // the previous call may still be reading the workspace on another stream
   CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
-  EventPair ep;
-  const int64_t launches_before = g_launches.load();
-  int rc = prof_open(c, s, &ep, 1);
+  ProfBracket prep;
+  int rc = prep.open(c, s, 1);
   if (rc) return rc;
   int64_t f16_b_off = 0;
-  if (mode == SPLIT_F16X2 && (rc = f16_scales(c, M, N, &f16_b_off))) { prof_abort(c, &ep); return rc; }
-  rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s, opA);
-  if (rc) { prof_abort(c, &ep); return rc; }
+  if (mode == SPLIT_F16X2 && (rc = f16_scales(c, M, N, &f16_b_off))) return rc;
+  if ((rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s, opA))) return rc;
   // clusters of two CTAs (256 x 128 tiles) when enabled and there are at least two 128-row blocks
   const bool pair = c.cta_pair && M > TC_BLOCK_M;
   if (b_ready) CUDA_TRY(cudaStreamWaitEvent(s, b_ready, 0));
-  rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, s, opB);
-  if (rc) { prof_abort(c, &ep); return rc; }
-  const int prep_launches = static_cast<int>(g_launches.load() - launches_before);
-  rc = prof_close(c, s, &ep, prep_launches);
-  if (rc) return rc;
+  if ((rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, s, opB))) return rc;
+  const int prep_launches = prep.launches();
+  if ((rc = prep.close())) return rc;
   const F16Scales f16{static_cast<const uint32_t *>(c.f16s.ptr), static_cast<const uint32_t *>(c.f16s.ptr) + f16_b_off};
   // (with profiling on, an event record sits between the last preparation kernel and the GEMM: no dependent launch then)
   rc = tc_run<OutT>(c, kind, M, N, K, alpha, ma, mb, beta, C, rsC, csC, pair, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
@@ -809,24 +778,12 @@ int prepack_dev(int which, void *dst, int64_t mn, int64_t k, const float *src, i
     if (classify(o, 4) != K_MAJOR) {
       // anything that is not K-major already (MN-major, general strides) is gathered into compact K-major rows first
       CUDA_TRY(cudaStreamWaitEvent(s, c->ws_free, 0));
-      const int64_t ld = round_up(k, 4);
       Buffer &g = c->gather[which];
-      if ((rc = ensure(g, static_cast<size_t>(mn) * ld * 4))) return rc;
-      const int64_t tiles = ((mn + 31) / 32) * ((k + 31) / 32);
-      const int read_along_r = (llabs(s_mn) < llabs(s_k)) ? 1 : 0;
-      pack_general_kernel<float, 0><<<grid_for(*c, tiles, 8), 256, 0, s>>>(src, mn, k, s_mn, s_k, static_cast<float *>(g.ptr),
-                                                                           nullptr, ld, read_along_r, OperandOp());
-      COUNT_LAUNCH();
-      CHECK_LAUNCH();
+      if ((rc = gather<float>(*c, o, g, nullptr, s))) return rc;
       rows = static_cast<const float *>(g.ptr);
-      rows_ld = ld;
+      rows_ld = round_up(k, 4);
     }
-    if (k <= 4 * 32 * F16ROWS_MAXV)
-      f16x2_rows_fused_kernel<32><<<grid_for(*c, (mn + 7) / 8, 4), 256, 0, s>>>(rows, mn, k, rows_ld, h, l, L.ld_b, amax, OperandOp());
-    else
-      f16x2_rows_fused_kernel<256><<<grid_for(*c, mn, 4), 256, 0, s>>>(rows, mn, k, rows_ld, h, l, L.ld_b, amax, OperandOp());
-    COUNT_LAUNCH();
-    CHECK_LAUNCH();
+    if ((rc = f16x2_rows(*c, rows, mn, k, rows_ld, h, l, L.ld_b, amax, s))) return rc;
     CUDA_TRY(cudaEventRecord(c->ws_free, s));
   }
   return finish(*c, static_cast<cudaStream_t>(stream), s);
@@ -868,14 +825,13 @@ int gemm_packed_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A
       if ((rc = packed_maps(c, packedA, M, K, TC_BLOCK_M, &ma, &f16.a))) return rc;
     } else {
       Operand oa{A, M, K, rsA, csA};
-      EventPair ep;
-      const int64_t before = g_launches.load();
       int64_t b_off = 0;
       if ((rc = f16_scales(c, M, 0, &b_off))) return rc;
-      if ((rc = prof_open(c, s, &ep, 1))) return rc;
-      if ((rc = prepare_operand<4>(c, oa, SPLIT_F16X2, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s))) { prof_abort(c, &ep); return rc; }
-      prep_launches = static_cast<int>(g_launches.load() - before);
-      if ((rc = prof_close(c, s, &ep, prep_launches))) return rc;
+      ProfBracket prep;
+      if ((rc = prep.open(c, s, 1))) return rc;
+      if ((rc = prepare_operand<4>(c, oa, SPLIT_F16X2, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s))) return rc;
+      prep_launches = prep.launches();
+      if ((rc = prep.close())) return rc;
       f16.a = static_cast<const uint32_t *>(c.f16s.ptr);
     }
     if ((rc = packed_maps(c, packedB, N, K, TC_BLOCK_N, &mb, &f16.b))) return rc;
@@ -935,12 +891,12 @@ int gemm_simt_ops(Ctx &c, int64_t M, int64_t N, int64_t K, float alpha, const fl
   CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
   int rc;
   if (opA) {
-    if ((rc = gather_op(c, Operand{A, M, K, rsA, csA}, *opA, c.gather[0], s, &A))) return rc;
-    rsA = round_up(K, 4); csA = 1;
+    if ((rc = gather<float>(c, Operand{A, M, K, rsA, csA}, c.gather[0], nullptr, s, opA))) return rc;
+    A = static_cast<const float *>(c.gather[0].ptr); rsA = round_up(K, 4); csA = 1;
   }
   if (opB) {
-    if ((rc = gather_op(c, Operand{B, N, K, csB, rsB}, *opB, c.gather[1], s, &B))) return rc;
-    rsB = 1; csB = round_up(K, 4);
+    if ((rc = gather<float>(c, Operand{B, N, K, csB, rsB}, c.gather[1], nullptr, s, opB))) return rc;
+    B = static_cast<const float *>(c.gather[1].ptr); rsB = 1; csB = round_up(K, 4);
   }
   if ((rc = gemm_simt<float>(c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi))) return rc;
   CUDA_TRY(cudaEventRecord(c.ws_free, s));
