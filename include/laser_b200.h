@@ -202,6 +202,37 @@ int laser_b200_gemm_strided_f32_fused_dev(int64_t M, int64_t N, int64_t K, float
                                           const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
                                           const laser_b200_epilogue *epi, int path, void *stream);
 
+/* ---- batched fused product -----------------------------------------------
+ * The batched twin of laser_b200_gemm_strided_f32_fused_dev: problem b (0 <= b < batch) computes
+ *   C_b <- act(alpha * opA(A_b) * opB(B_b) + beta * C_b + bias),   X_b = X + b * batchStrides->X
+ * for every operand X (A, B, C and the aux tensors of opA / opB).  The reference's roadmap names batched products ("N tensors
+ * A multiplied by a tensor B, or N tensors A multiplied by N tensors B") and small products (README.md:253-263): small
+ * problems in large batches -- per-sample or per-head products, a convolution image by image -- fill the GPU only together.
+ * Each operand is prepared for the whole batch in as many launches as one problem's operand, and one GEMM launch runs the
+ * tiles of every problem.
+ *   Strides are in elements and may be negative.  A stride of 0 shares A (or B) across the batch: it is prepared once.
+ *   C may not be shared, and different problems' outputs must not overlap.  The bias vector is shared by every problem.
+ *   Every problem takes the path one fused call with an op would take for its shape (PATH_AUTO never takes the N <= 4 GEMV
+ *   shortcut), and the whole batch takes that one path; each problem's C is bit for bit what that single call gives.
+ *   batch == 1 is exactly laser_b200_gemm_strided_f32_fused_dev.  batch == 0, or M, N or K == 0: LASER_B200_OK, nothing is
+ *   launched and C is untouched.
+ *   LASER_B200_EINVAL, before anything is launched: batch < 0; batchStrides == NULL with batch > 0; batchStrides->C == 0 with
+ *   batch > 1; an unknown op, or a derivative op without aux; an unknown path.
+ *   LASER_B200_CTA_PAIR does not apply: batched launches use single CTAs.  A batch whose prepared operands would exceed
+ *   LASER_B200_BATCH_WS_MB megabytes (read at initialisation, default 1024) runs in chunks of whole problems, one preparation
+ *   and one GEMM launch sequence per chunk. */
+typedef struct {
+  int64_t A, B, C;    /* element offset between consecutive problems; 0 shares A (or B) across the batch */
+  int64_t auxA, auxB; /* the same for opA->aux / opB->aux (ignored without a derivative op) */
+} laser_b200_batch_strides;
+int laser_b200_gemm_strided_batched_f32_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha,
+                                                  const float *A, int64_t rowStrideA, int64_t colStrideA,
+                                                  const float *B, int64_t rowStrideB, int64_t colStrideB,
+                                                  float beta, float *C, int64_t rowStrideC, int64_t colStrideC,
+                                                  const laser_b200_batch_strides *batchStrides,
+                                                  const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
+                                                  const laser_b200_epilogue *epi, int path, void *stream);
+
 /* ---- pre-packed operands (device) -----------------------------------------
  * Replaces  gemm_prepackA_mem_required / gemm_prepackB_mem_required, gemm_prepackA / gemm_prepackB
  * and gemm_packed   (laser/primitives/matrix_multiplication/gemm_prepacked.nim:63-292).

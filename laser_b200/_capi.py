@@ -33,6 +33,10 @@ class OperandOp(ctypes.Structure):
     _fields_ = [("op", i32), ("aux", vp), ("auxRowStride", i64), ("auxColStride", i64)]
 
 
+class BatchStrides(ctypes.Structure):
+    _fields_ = [("A", i64), ("B", i64), ("C", i64), ("auxA", i64), ("auxB", i64)]
+
+
 OP_NONE, OP_RELU, OP_TANH, OP_SIGMOID, OP_RELU_GRAD, OP_TANH_GRAD, OP_SIGMOID_GRAD = 0, 1, 2, 3, 4, 5, 6
 OP_NAMES = {"none": 0, "relu": 1, "tanh": 2, "sigmoid": 3, "relu_grad": 4, "tanh_grad": 5, "sigmoid_grad": 6}
 
@@ -68,6 +72,8 @@ SIGNATURES = {
     "laser_b200_gemm_strided_f32_epi_dev": (ctypes.c_int, _gemm_sig(f32) + [ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
     "laser_b200_gemm_strided_f32_fused_dev": (ctypes.c_int, _gemm_sig(f32) + [ctypes.POINTER(OperandOp), ctypes.POINTER(OperandOp),
                                                                               ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
+    "laser_b200_gemm_strided_batched_f32_fused_dev": (ctypes.c_int, [i64] + _gemm_sig(f32) + [
+        ctypes.POINTER(BatchStrides), ctypes.POINTER(OperandOp), ctypes.POINTER(OperandOp), ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
     "laser_b200_gemm_strided_f64_dev": (ctypes.c_int, _gemm_sig(f64) + [vp]),
     "laser_b200_gemm_strided_i32_dev": (ctypes.c_int, _gemm_sig(i32) + [vp]),
     "laser_b200_gemm_strided_i64_dev": (ctypes.c_int, _gemm_sig(i64) + [vp]),

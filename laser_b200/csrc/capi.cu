@@ -81,9 +81,11 @@ struct MapKey {
   const void *base;
   int64_t inner, outer, stride;
   int esz, box_inner, box_outer, swz;
+  int64_t depth, depth_stride;   // rank 3 (batched launches): matrices and their distance in elements; depth 0: rank 2
   bool operator==(const MapKey &o) const {
     return base == o.base && inner == o.inner && outer == o.outer && stride == o.stride && esz == o.esz &&
-           box_inner == o.box_inner && box_outer == o.box_outer && swz == o.swz;
+           box_inner == o.box_inner && box_outer == o.box_outer && swz == o.swz && depth == o.depth &&
+           depth_stride == o.depth_stride;
   }
 };
 struct MapCacheEntry {
@@ -114,6 +116,8 @@ struct Ctx {
   int kc_faithful = 128;
   bool dyn_sched = true;  // env LASER_B200_DYNSCHED=0: static round-robin tiles instead of the atomic counter
   bool pdl = true;        // env LASER_B200_PDL=0: ordinary launch of the GEMM kernel after the preparation kernels
+  // env LASER_B200_BATCH_WS_MB: prepared workspace of one batched call at most; a larger batch runs in chunks of whole problems
+  int64_t batch_ws_bytes = static_cast<int64_t>(1024) << 20;
   bool profiling = false;
   std::vector<EventPair> prof;
   int dev = -1;
@@ -195,6 +199,10 @@ int get_ctx(Ctx **out) {
       if (const char *pt = getenv("LASER_B200_PANEL_TAPER")) c.panel_taper = atoi(pt) != 0;
       if (const char *ds = getenv("LASER_B200_DYNSCHED")) c.dyn_sched = atoi(ds) != 0;
       if (const char *pd = getenv("LASER_B200_PDL")) c.pdl = atoi(pd) != 0;
+      if (const char *bw = getenv("LASER_B200_BATCH_WS_MB")) {
+        const int64_t v = atoll(bw);
+        if (v >= 1) c.batch_ws_bytes = v << 20;
+      }
       if (const char *pr = getenv("LASER_B200_PANEL_ROWS")) {
         const int64_t v = atoll(pr) / 256 * 256;   // whole CTA-pair tiles
         if (v >= 256) c.panel_rows = v;
@@ -368,6 +376,9 @@ int gemm_simt(Ctx &c, int64_t M, int64_t N, int64_t K, T alpha, const T *A, int6
 struct Operand {
   const void *ptr;
   int64_t mn, k, s_mn, s_k;
+  // batched launch: `batch` problems s_b elements apart (the aux of their op: aux_sb apart), read through rank-3 tensor maps;
+  // batch 1 with a batched launch is an operand the problems share.  0: a single problem, rank-2 maps.
+  int64_t batch = 0, s_b = 0, aux_sb = 0;
 };
 enum Major { K_MAJOR = 0, MN_MAJOR = 1, GENERAL = 2 };
 
@@ -381,20 +392,22 @@ Major classify(const Operand &o, int esz) {
 }
 
 int encode_map(Ctx &c, CUtensorMap *map, int esz, const void *base, int64_t inner, int64_t outer,
-               int64_t outer_stride_elems, int box_inner, int box_outer, CUtensorMapSwizzle swz) {
-  const MapKey key{base, inner, outer, outer_stride_elems, esz, box_inner, box_outer, static_cast<int>(swz)};
+               int64_t outer_stride_elems, int box_inner, int box_outer, CUtensorMapSwizzle swz, int64_t depth = 0,
+               int64_t depth_stride = 0) {
+  const MapKey key{base, inner, outer, outer_stride_elems, esz, box_inner, box_outer, static_cast<int>(swz), depth, depth_stride};
   for (int i = 0; i < kMapCacheSize; ++i)
     if (c.map_cache[i].valid && c.map_cache[i].key == key) {
       *map = c.map_cache[i].map;
       return LASER_B200_OK;
     }
-  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(inner), static_cast<cuuint64_t>(outer)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(outer_stride_elems) * esz};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(box_inner), static_cast<cuuint32_t>(box_outer)};
-  const cuuint32_t estr[2] = {1, 1};
+  // rank 3: {inner, outer, depth} with a box depth of 1 -- one matrix of a batch per load, zero-filled at its own edges
+  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(inner), static_cast<cuuint64_t>(outer), static_cast<cuuint64_t>(depth)};
+  const cuuint64_t strides[2] = {static_cast<cuuint64_t>(outer_stride_elems) * esz, static_cast<cuuint64_t>(depth_stride) * esz};
+  const cuuint32_t box[3] = {static_cast<cuuint32_t>(box_inner), static_cast<cuuint32_t>(box_outer), 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
   // 16-bit tiles travel as BFLOAT16 whatever their format (bf16 / fp16): TMA only moves the words
   const CUtensorMapDataType dt = esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  CUresult r = c.encode(map, dt, 2, const_cast<void *>(base), dims, strides, box, estr,
+  CUresult r = c.encode(map, dt, depth > 0 ? 3 : 2, const_cast<void *>(base), dims, strides, box, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
@@ -411,15 +424,16 @@ int encode_map(Ctx &c, CUtensorMap *map, int esz, const void *base, int64_t inne
 }
 
 // tensor map for one operand given as compact/strided [mn][k] data with the stated major-ness
+// (depth > 0: rank 3 over `depth` such operands depth_stride elements apart)
 int operand_map(Ctx &c, CUtensorMap *map, int esz, const void *base, Major major, int64_t mn,
-                int64_t k, int64_t ld, int block_mn) {
+                int64_t k, int64_t ld, int block_mn, int64_t depth = 0, int64_t depth_stride = 0) {
   const int block_k = TC_ROW_BYTES / esz;
   const int mn_atom = TC_ROW_BYTES / esz;
   if (major == K_MAJOR)
-    return encode_map(c, map, esz, base, k, mn, ld, block_k, block_mn, CU_TENSOR_MAP_SWIZZLE_128B);
+    return encode_map(c, map, esz, base, k, mn, ld, block_k, block_mn, CU_TENSOR_MAP_SWIZZLE_128B, depth, depth_stride);
   // MN-major fp32/tf32 tiles need the 32-byte-atom flavour of the 128B swizzle (see ptx.cuh)
   return encode_map(c, map, esz, base, mn, k, ld, mn_atom, block_k,
-                    esz == 4 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B);
+                    esz == 4 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, depth, depth_stride);
 }
 
 // Tensor maps of one operand for the tensor-core kernel: piece 0 = the operand itself (one pass) or its high piece,
@@ -453,87 +467,100 @@ inline bool op_same_layout(const Operand &o, const OperandOp &op) {
 }
 
 // ---- the preparation steps: one function, and one launch site, per kernel family of split.cuh ----
-// A step takes its op as a pointer (nullptr: none) and hands `launch` either (std::true_type, *op) or
-// (std::false_type, OperandOp()): the kernel's HAS_OP and plain instantiations come from the same launch statement.
+// A step takes its op as a pointer (nullptr: none) and its problems as a Batch (n == 1: one problem), and hands `launch`
+// (has_op, op, batched): has_op is std::true_type with *op or std::false_type with OperandOp(), batched is std::true_type
+// when bt.n > 1.  The kernel's plain, HAS_OP and BATCHED instantiations come from the same launch statement.
 template <typename Launch>
-int launch_prep(const OperandOp *op, Launch launch) {
-  if (op) launch(std::true_type(), *op);
-  else launch(std::false_type(), OperandOp());
+int launch_prep(const OperandOp *op, const Batch &bt, Launch launch) {
+  auto with_op = [&](auto batched) {
+    if (op) launch(std::true_type(), *op, batched);
+    else launch(std::false_type(), OperandOp(), batched);
+  };
+  if (bt.n > 1) with_op(std::true_type());
+  else with_op(std::false_type());
   COUNT_LAUNCH();
   CHECK_LAUNCH();
   return LASER_B200_OK;
 }
+// the problems an operand's preparation covers (an operand the batch shares: one)
+inline Batch batch_of(const Operand &o) { return Batch{o.batch > 1 ? o.batch : 1, o.s_b, o.aux_sb}; }
 
 // The gather: op(operand), or the operand itself, from any strides into compact K-major rows [mn][round_up(k, 16 / sizeof(T))]
 // allocated in dst (aux read with its own strides).  MODE 1 (fp32): the tf32 hi / lo pieces into dst / *lo.  bf16 operands
 // carry no op.
+// A batched operand: the problems' rows stacked, [batch][mn][ld].
 template <typename T, int MODE = 0>
 int gather(Ctx &c, const Operand &o, Buffer &dst, Buffer *lo, cudaStream_t s, const OperandOp *op = nullptr) {
+  const Batch bt = batch_of(o);
   const int64_t ld = round_up(o.k, 16 / static_cast<int64_t>(sizeof(T)));
-  const size_t bytes = static_cast<size_t>(o.mn) * ld * sizeof(T);
+  const size_t bytes = static_cast<size_t>(bt.n * o.mn) * ld * sizeof(T);
   int rc;
   if ((rc = ensure(dst, bytes))) return rc;
   if (MODE == 1 && (rc = ensure(*lo, bytes))) return rc;
-  const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32);
+  const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32) * bt.n;
   const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
   T *d0 = static_cast<T *>(dst.ptr), *d1 = MODE == 1 ? static_cast<T *>(lo->ptr) : nullptr;
-  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
-    pack_general_kernel<T, MODE, decltype(has_op)::value && sizeof(T) == 4><<<grid_for(c, tiles, 8), 256, 0, s>>>(
-        static_cast<const T *>(o.ptr), o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, k);
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
+    constexpr bool HAS_OP = decltype(has_op)::value && sizeof(T) == 4, BATCHED = decltype(batched)::value && sizeof(T) == 4;
+    pack_general_kernel<T, MODE, HAS_OP, BATCHED><<<grid_for(c, tiles, 8), 256, 0, s>>>(
+        static_cast<const T *>(o.ptr), o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, k, bt);
   });
 }
 
 // TF32X3 in place: tf32 hi / lo pieces [R][ld] of fp32 rows [R][Cc], src_ld apart
 int tf32_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, float *hi, float *lo, int64_t ld, cudaStream_t s,
-               const OperandOp *op) {
-  const int64_t items = R * ((Cc + 3) / 4);
-  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
-    split_rows_tf32_kernel<decltype(has_op)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
-        src, R, Cc, src_ld, hi, lo, ld, k);
+               const OperandOp *op, const Batch &bt = Batch()) {
+  const int64_t items = bt.n * R * ((Cc + 3) / 4);
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
+    split_rows_tf32_kernel<decltype(has_op)::value, decltype(batched)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
+        src, R, Cc, src_ld, hi, lo, ld, k, bt);
   });
 }
 
 // F16X3, one scale per row of fp32 rows [R][Cc] (src_ld apart): the abs-max word of each row, the scale and the two fp16
 // pieces [R][ld_b] in ONE pass (split.cuh).  Rows of up to 1024 floats: a warp per row.  Longer rows: prefetched into a
 // shared-memory ring by the copy engine when they allow it (16-byte aligned, at most 8192 floats; the ring kernel has no op
-// variant), the CTA per row otherwise.
+// variant, nor a batched one), the CTA per row otherwise.
 int f16x2_rows(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *hb, uint16_t *lb, int64_t ld_b,
-               uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
-  const bool ring = !op && f16x2_rows_ring_ok(src, Cc, src_ld);
+               uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr, const Batch &bt = Batch()) {
+  const bool ring = !op && bt.n == 1 && f16x2_rows_ring_ok(src, Cc, src_ld);
   if (ring && !c.ring_attr_set) {
     CUDA_TRY(cudaFuncSetAttribute(f16x2_rows_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(f16x2_rows_ring_smem(4 * 256 * F16ROWS_MAXV))));
     c.ring_attr_set = true;
   }
-  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
-    constexpr bool HAS_OP = decltype(has_op)::value;
+  const int64_t rows = bt.n * R;
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
+    constexpr bool HAS_OP = decltype(has_op)::value, BATCHED = decltype(batched)::value;
     if (Cc <= 4 * 32 * F16ROWS_MAXV)
-      f16x2_rows_fused_kernel<32, HAS_OP><<<grid_for(c, (R + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words, k);
+      f16x2_rows_fused_kernel<32, HAS_OP, BATCHED><<<grid_for(c, (rows + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b,
+                                                                                             words, k, bt);
     else if (ring)
       f16x2_rows_ring_kernel<<<grid_for(c, R, 2), 256, f16x2_rows_ring_smem(Cc), s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words);
     else
-      f16x2_rows_fused_kernel<256, HAS_OP><<<grid_for(c, R, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words, k);
+      f16x2_rows_fused_kernel<256, HAS_OP, BATCHED><<<grid_for(c, rows, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words, k,
+                                                                                        bt);
   });
 }
 
 // F16X3, one scale per column of fp32 rows [R][Cc]: the abs-max word of every column (zeroed here, then strip reductions
 // combined by atomicMax).  A column's scale needs the whole column, so the split is a second pass.
 int f16x2_col_scales(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint32_t *words, cudaStream_t s,
-                     const OperandOp *op = nullptr) {
-  CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(Cc) * sizeof(uint32_t), s));
-  const int64_t items = ((Cc + 3) / 4) * ((R + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS);
-  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
-    absmax_mn_kernel<true, decltype(has_op)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
-        src, R, Cc, src_ld, words, k);
+                     const OperandOp *op = nullptr, const Batch &bt = Batch()) {
+  CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(bt.n * Cc) * sizeof(uint32_t), s));
+  const int64_t items = ((Cc + 3) / 4) * ((R + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS) * bt.n;
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
+    absmax_mn_kernel<true, decltype(has_op)::value, decltype(batched)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
+        src, R, Cc, src_ld, words, k, bt);
   });
 }
 // F16X3, one scale per column: the two fp16 pieces [R][ld_b] of fp32 rows [R][Cc] against the columns' scale words
 int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *hb, uint16_t *lb, int64_t ld_b,
-                    const uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
-  const int64_t items = ((Cc + 255) / 256) * ((R + SPLIT_ROWS - 1) / SPLIT_ROWS);
-  return launch_prep(op, [&](auto has_op, const OperandOp &k) {
-    split_rows_f16x2_kernel<true, decltype(has_op)::value><<<grid_for(c, items, 8), 256, 0, s>>>(
-        src, R, Cc, src_ld, hb, lb, ld_b, words, k);
+                    const uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr, const Batch &bt = Batch()) {
+  const int64_t items = ((Cc + 255) / 256) * ((R + SPLIT_ROWS - 1) / SPLIT_ROWS) * bt.n;
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
+    split_rows_f16x2_kernel<true, decltype(has_op)::value, decltype(batched)::value><<<grid_for(c, items, 8), 256, 0, s>>>(
+        src, R, Cc, src_ld, hb, lb, ld_b, words, k, bt);
   });
 }
 
@@ -544,21 +571,30 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
 //   Anything else: one gather, which applies the op, into compact K-major rows.  TMA reads those (bf16, TF32X1), the gather
 //     splits them on the way (TF32X3), or the plain row kernel prepares them (F16X3).
 // wgmma reads tf32 tiles K-major only, and TMA applies no op.  op: nullptr, or an operand op (fp32 operands only).
+// A batched operand (o.batch > 0) is prepared in the same launches, every problem's pieces and scale words stacked; its
+// maps are rank 3.  It is read in place only where every problem is: TMA needs a positive batch stride of whole 16-byte
+// units, the preparation kernels 16-byte aligned rows (operand and aux) in every problem.
 template <int ESZ>
 int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w, int block_mn,
                     OperandMaps *m, bool *used_ws, cudaStream_t s, const OperandOp *op = nullptr) {
   const Major mj = classify(o, ESZ);
-  const bool tma_layout = mj == K_MAJOR || (mj == MN_MAJOR && (ESZ == 2 || mode == SPLIT_F16X2));
-  const bool in_place = tma_layout && (!op || (mode != SPLIT_NONE && op_same_layout(o, *op)));
+  const Batch bt = batch_of(o);
+  const bool rows_ok = bt.n == 1 || ((o.s_b * ESZ) % 16 == 0 && (!op || !op->aux || o.aux_sb % 4 == 0));
+  const bool map_ok = bt.n == 1 || (o.s_b > 0 && o.s_b < (static_cast<int64_t>(1) << 40) / ESZ);
+  const bool tma_layout = (mj == K_MAJOR || (mj == MN_MAJOR && (ESZ == 2 || mode == SPLIT_F16X2))) && rows_ok;
+  const bool in_place = tma_layout && (mode == SPLIT_NONE ? !op && map_ok : !op || op_same_layout(o, *op));
   const Major out_mj = in_place ? mj : K_MAJOR;              // layout of the arrays the tensor-core kernel reads
   const int64_t R = (out_mj == K_MAJOR) ? o.mn : o.k;        // their rows
   const int64_t Cc = (out_mj == K_MAJOR) ? o.k : o.mn;       // their contiguous extent
   const int64_t src_ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;   // row pitch of the operand, read in place
   const int64_t ld = round_up(Cc, 16 / ESZ);
+  // rank-3 maps of a batched launch: `depth` matrices (1: shared by the batch) `d_stride(pitch)` elements apart
+  const int64_t depth = o.batch > 0 ? bt.n : 0;
+  auto d_stride = [&](int64_t pitch) { return bt.n > 1 ? (in_place && mode == SPLIT_NONE ? o.s_b : R * pitch) : R * pitch; };
   m->mn_major = (out_mj == MN_MAJOR);
   int rc;
   if (mode == SPLIT_NONE && in_place) {
-    if ((rc = operand_map(c, &m->p0, ESZ, o.ptr, mj, o.mn, o.k, src_ld, block_mn))) return rc;
+    if ((rc = operand_map(c, &m->p0, ESZ, o.ptr, mj, o.mn, o.k, src_ld, block_mn, depth, d_stride(src_ld)))) return rc;
     m->p1 = m->p0;
     return LASER_B200_OK;
   }
@@ -571,39 +607,39 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
     const OperandOp *on_load = (in_place && op) ? &kop : nullptr;
     if (mode == SPLIT_F16X2) {
       const int64_t ld_b = round_up(Cc, 8);
-      const size_t bytes_b = static_cast<size_t>(R) * ld_b * 2;
+      const size_t bytes_b = static_cast<size_t>(bt.n * R) * ld_b * 2;
       if ((rc = ensure(*w.p0, bytes_b))) return rc;
       if ((rc = ensure(*w.p1, bytes_b))) return rc;
-      if (c.f16s.bytes < static_cast<size_t>(w.amax_off + o.mn) * sizeof(uint32_t))
+      if (c.f16s.bytes < static_cast<size_t>(w.amax_off + bt.n * o.mn) * sizeof(uint32_t))
         return set_error(LASER_B200_ECUDA, "internal: F16X3 scale buffer not sized for this operand");
       uint16_t *hb = static_cast<uint16_t *>(w.p0->ptr), *lb = static_cast<uint16_t *>(w.p1->ptr);
       uint32_t *words = static_cast<uint32_t *>(c.f16s.ptr) + w.amax_off;
-      if (!in_place) {
+      if (!in_place) {   // the gathered problems are stacked rows: one plain row pass over all of them
         if ((rc = gather<float>(c, o, *w.gather, nullptr, s, op))) return rc;
-        rc = f16x2_rows(c, static_cast<const float *>(w.gather->ptr), R, Cc, ld, hb, lb, ld_b, words, s);
+        rc = f16x2_rows(c, static_cast<const float *>(w.gather->ptr), bt.n * R, Cc, ld, hb, lb, ld_b, words, s);
       } else if (out_mj == K_MAJOR) {
-        rc = f16x2_rows(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load);
+        rc = f16x2_rows(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load, bt);
       } else {
-        if ((rc = f16x2_col_scales(c, src, R, Cc, src_ld, words, s, on_load))) return rc;
-        rc = f16x2_col_split(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load);
+        if ((rc = f16x2_col_scales(c, src, R, Cc, src_ld, words, s, on_load, bt))) return rc;
+        rc = f16x2_col_split(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load, bt);
       }
       if (rc) return rc;
-      if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, o.k, ld_b, block_mn))) return rc;
-      return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, o.k, ld_b, block_mn);
+      if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, o.k, ld_b, block_mn, depth, d_stride(ld_b)))) return rc;
+      return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, o.k, ld_b, block_mn, depth, d_stride(ld_b));
     }
     if (!in_place) {
       rc = (mode == SPLIT_TF32) ? gather<float, 1>(c, o, *w.p0, w.p1, s, op) : gather<float>(c, o, *w.p0, nullptr, s, op);
     } else {   // TF32X3, K-major
-      const size_t bytes = static_cast<size_t>(R) * ld * sizeof(float);
+      const size_t bytes = static_cast<size_t>(bt.n * R) * ld * sizeof(float);
       if ((rc = ensure(*w.p0, bytes))) return rc;
       if ((rc = ensure(*w.p1, bytes))) return rc;
-      rc = tf32_split(c, src, R, Cc, src_ld, static_cast<float *>(w.p0->ptr), static_cast<float *>(w.p1->ptr), ld, s, on_load);
+      rc = tf32_split(c, src, R, Cc, src_ld, static_cast<float *>(w.p0->ptr), static_cast<float *>(w.p1->ptr), ld, s, on_load, bt);
     }
     if (rc) return rc;
   }
-  if ((rc = operand_map(c, &m->p0, ESZ, w.p0->ptr, out_mj, o.mn, o.k, ld, block_mn))) return rc;
+  if ((rc = operand_map(c, &m->p0, ESZ, w.p0->ptr, out_mj, o.mn, o.k, ld, block_mn, depth, d_stride(ld)))) return rc;
   m->p1 = m->p0;
-  if (mode == SPLIT_TF32) return operand_map(c, &m->p1, ESZ, w.p1->ptr, out_mj, o.mn, o.k, ld, block_mn);
+  if (mode == SPLIT_TF32) return operand_map(c, &m->p1, ESZ, w.p1->ptr, out_mj, o.mn, o.k, ld, block_mn, depth, d_stride(ld));
   return LASER_B200_OK;
 }
 
@@ -625,11 +661,19 @@ inline TcKind tc_kind_of_path(int path) {
 }
 inline SplitMode split_mode(TcKind k) { return k == TC_TF32X3 ? SPLIT_TF32 : k == TC_F16X3 ? SPLIT_F16X2 : SPLIT_NONE; }
 
-// launch the tensor-core kernel on prepared operands (c.mu held by the caller)
+// a batched call: `batch` problems, operand X of problem b at X + b * X_stride (0: the batch shares it)
+struct BatchArgs {
+  int64_t batch;
+  int64_t A, B, C, auxA, auxB;
+};
+
+// launch the tensor-core kernel on prepared operands (c.mu held by the caller).  bat: a batched launch (tc_params.h; the maps
+// are rank 3, single CTAs), with a_shared / b_shared for operands prepared once for the whole batch.
 template <typename OutT>
 int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, const OperandMaps &ma,
            const OperandMaps &mb, float beta, OutT *C, int64_t rsC, int64_t csC, bool pair, cudaStream_t s,
-           const Epilogue &epi, const F16Scales *f16 = nullptr, bool after_prep = false) {
+           const Epilogue &epi, const F16Scales *f16 = nullptr, bool after_prep = false, const BatchArgs *bat = nullptr,
+           bool a_shared = false, bool b_shared = false) {
   TcLaunch l;
   l.a0 = ma.p0; l.a1 = ma.p1; l.b0 = mb.p0; l.b1 = mb.p1;
   l.a_mn = ma.mn_major; l.b_mn = mb.mn_major;
@@ -640,6 +684,15 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
   p.M = M; p.N = N; p.K = K; p.alpha = alpha; p.beta = beta;
   p.C = C; p.rsC = rsC; p.csC = csC; p.zero = 0; p.epi = epi;
   if (f16) { p.amax_a = f16->a; p.amax_b = f16->b; }
+  if (bat) {
+    l.batched = true;
+    p.batch = static_cast<int>(bat->batch);
+    p.map_b_a = a_shared ? 0 : 1;
+    p.map_b_b = b_shared ? 0 : 1;
+    p.bsC = bat->C;
+    p.amax_bs_a = a_shared ? 0 : M;
+    p.amax_bs_b = b_shared ? 0 : N;
+  }
   const int npass = (kind == TC_TF32X3 || kind == TC_F16X3) ? 3 : 1;
   const TcPlanCfg cfg{c.kc_faithful, c.raster_g, c.splitk_enabled, c.sm_count};
   if (kind == TC_BF16 || kind == TC_F16X3) tc_plan<2, std::is_same<OutT, float>::value>(p, npass, pair, cfg);
@@ -676,12 +729,16 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
       if ((rc = ensure(c.splitk, static_cast<size_t>(ws_floats) * sizeof(float)))) return rc;
       p.split_ws = static_cast<float *>(c.splitk.ptr);
       if ((rc = launch(l))) return rc;
-      const int n_tail = p.num_m_blocks * p.num_n_blocks - p.n_direct;
+      const int n_tail = p.num_m_blocks * p.num_n_blocks * p.batch - p.n_direct;
       const int tile_m = pair ? 2 * TC_BLOCK_M : TC_BLOCK_M;
       const int64_t items = (static_cast<int64_t>(n_tail) * tile_m * (TC_BLOCK_N / 4) + 255) / 256;
-      splitk_tail_reduce_kernel<<<grid_for(c, items, 8), 256, 0, s>>>(
-          static_cast<const float *>(c.splitk.ptr), p.k_splits, n_tail, p.n_direct, p.num_m_blocks, p.num_n_blocks, p.raster_g,
-          tile_m, M, N, alpha, beta, C, rsC, csC, p.epi.bias, p.epi.bias_per_row, p.epi.act);
+      auto reduce = [&](auto batched) {
+        splitk_tail_reduce_kernel<decltype(batched)::value><<<grid_for(c, items, 8), 256, 0, s>>>(
+            static_cast<const float *>(c.splitk.ptr), p.k_splits, n_tail, p.n_direct, p.num_m_blocks, p.num_n_blocks, p.raster_g,
+            tile_m, M, N, alpha, beta, C, rsC, csC, p.epi.bias, p.epi.bias_per_row, p.epi.act, p.bsC);
+      };
+      if (bat) reduce(std::true_type());
+      else reduce(std::false_type());
       COUNT_LAUNCH();
       CHECK_LAUNCH();
       CUDA_TRY(cudaEventRecord(c.ws_free, s));  // the planes are workspace too
@@ -697,7 +754,7 @@ template <int SRC_ESZ, typename OutT>
 int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, const void *A, int64_t rsA,
             int64_t csA, const void *B, int64_t rsB, int64_t csB, float beta, OutT *C, int64_t rsC,
             int64_t csC, cudaStream_t s, const Epilogue &epi, cudaEvent_t b_ready = nullptr, const OperandOp *opA = nullptr,
-            const OperandOp *opB = nullptr) {
+            const OperandOp *opB = nullptr, const BatchArgs *bat = nullptr) {
   // b_ready: B becomes valid only when this event has fired (the row-sharded driver: B is in flight on the communication
   // stream); everything that does not read B -- the preparation of A -- is queued before the wait.
   // opA / opB: operand ops applied while the operands are prepared (fp32 only)
@@ -707,6 +764,13 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   const SplitMode mode = split_mode(kind);
   Operand oa{A, M, K, rsA, csA};
   Operand ob{B, N, K, csB, rsB};
+  // bat: every problem's operand in the same launches (an operand -- op included -- that the batch shares: prepared once)
+  const bool a_shared = bat && bat->A == 0 && (!opA || !opA->aux || bat->auxA == 0);
+  const bool b_shared = bat && bat->B == 0 && (!opB || !opB->aux || bat->auxB == 0);
+  if (bat) {
+    oa.batch = a_shared ? 1 : bat->batch; oa.s_b = bat->A; oa.aux_sb = bat->auxA;
+    ob.batch = b_shared ? 1 : bat->batch; ob.s_b = bat->B; ob.aux_sb = bat->auxB;
+  }
   OperandMaps ma, mb;
   bool used_ws = false;
   // the previous call may still be reading the workspace on another stream
@@ -715,10 +779,12 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   int rc = prep.open(c, s, 1);
   if (rc) return rc;
   int64_t f16_b_off = 0;
-  if (mode == SPLIT_F16X2 && (rc = f16_scales(c, M, N, &f16_b_off))) return rc;
+  if (mode == SPLIT_F16X2 &&
+      (rc = f16_scales(c, batch_of(oa).n * M, batch_of(ob).n * N, &f16_b_off)))
+    return rc;
   if ((rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s, opA))) return rc;
-  // clusters of two CTAs (256 x 128 tiles) when enabled and there are at least two 128-row blocks
-  const bool pair = c.cta_pair && M > TC_BLOCK_M;
+  // clusters of two CTAs (256 x 128 tiles) when enabled and there are at least two 128-row blocks (never in a batched launch)
+  const bool pair = !bat && c.cta_pair && M > TC_BLOCK_M;
   if (b_ready) CUDA_TRY(cudaStreamWaitEvent(s, b_ready, 0));
   if ((rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, s, opB))) return rc;
   const int prep_launches = prep.launches();
@@ -726,7 +792,7 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   const F16Scales f16{static_cast<const uint32_t *>(c.f16s.ptr), static_cast<const uint32_t *>(c.f16s.ptr) + f16_b_off};
   // (with profiling on, an event record sits between the last preparation kernel and the GEMM: no dependent launch then)
   rc = tc_run<OutT>(c, kind, M, N, K, alpha, ma, mb, beta, C, rsC, csC, pair, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
-                    prep_launches > 0 && !c.profiling);
+                    prep_launches > 0 && !c.profiling, bat, a_shared, b_shared);
   if (rc) return rc;
   if (used_ws) CUDA_TRY(cudaEventRecord(c.ws_free, s));
   return LASER_B200_OK;
@@ -1022,6 +1088,111 @@ int operand_op_of(const laser_b200_operand_op *in, bool is_b, OperandOp *op, con
   op->aux_sc = is_b ? in->auxRowStride : in->auxColStride;
   *out = op;
   return LASER_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+//              batched fused product: the problems of a batch in one GEMM launch
+// ---------------------------------------------------------------------------------------
+// An operand -- with its op -- is the same in every problem: prepared once, read by every problem
+inline bool batch_shares(int64_t stride, const OperandOp *op, int64_t aux_stride) {
+  return stride == 0 && (!op || !op->aux || aux_stride == 0);
+}
+
+// workspace one problem of a batched call prepares on `path` (bytes, an upper bound): the pieces, gather copy and scale words
+// of each operand the problems do not share
+int64_t batch_ws_per_problem(int path, int64_t M, int64_t N, int64_t K, bool a_own, bool b_own, bool opA, bool opB) {
+  auto one = [&](int64_t mn, bool has_op) -> int64_t {
+    const int64_t g = mn * round_up(K, 4) * 4;   // a compact fp32 copy, or one tf32 piece
+    if (path == LASER_B200_PATH_F16X3) return 2 * mn * round_up(K, 8) * 2 + g + mn * 4;
+    if (path == LASER_B200_PATH_TF32X3) return 2 * g;
+    if (path == LASER_B200_PATH_TF32X1) return g;
+    return has_op ? g : 0;   // exact path: the op'd operand
+  };
+  return (a_own ? one(M, opA) : 0) + (b_own ? one(N, opB) : 0);
+}
+
+// problems [0, bat.batch) of a batched call on the resolved path: one preparation launch per step and operand, one GEMM launch
+int batched_run(Ctx &c, int path, const BatchArgs &bat, int64_t M, int64_t N, int64_t K, float alpha, const float *A,
+                int64_t rsA, int64_t csA, const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC,
+                int64_t csC, cudaStream_t s, const Epilogue &epi, const OperandOp *opA, const OperandOp *opB) {
+  if (path != LASER_B200_PATH_SIMT)
+    return gemm_tc<4, float>(c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, nullptr,
+                             opA, opB, &bat);
+  int64_t bsA = bat.A, bsB = bat.B;
+  if (!opA && !opB)
+    return gemm_simt<float>(c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, bat.batch, bsA, bsB, bat.C);
+  // exact path with ops: the batched gather materialises every problem's op'd operand (gemm_simt_ops, batched)
+  std::lock_guard<std::mutex> lk(c.mu);
+  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
+  int rc;
+  if (opA) {
+    const bool shared = batch_shares(bat.A, opA, bat.auxA);
+    if ((rc = gather<float>(c, Operand{A, M, K, rsA, csA, shared ? 1 : bat.batch, bat.A, bat.auxA}, c.gather[0], nullptr, s, opA)))
+      return rc;
+    A = static_cast<const float *>(c.gather[0].ptr); rsA = round_up(K, 4); csA = 1; bsA = shared ? 0 : M * rsA;
+  }
+  if (opB) {
+    const bool shared = batch_shares(bat.B, opB, bat.auxB);
+    if ((rc = gather<float>(c, Operand{B, N, K, csB, rsB, shared ? 1 : bat.batch, bat.B, bat.auxB}, c.gather[1], nullptr, s, opB)))
+      return rc;
+    B = static_cast<const float *>(c.gather[1].ptr); rsB = 1; csB = round_up(K, 4); bsB = shared ? 0 : N * csB;
+  }
+  if ((rc = gemm_simt<float>(c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, bat.batch, bsA, bsB, bat.C)))
+    return rc;
+  CUDA_TRY(cudaEventRecord(c.ws_free, s));
+  return LASER_B200_OK;
+}
+
+int batched_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
+                      const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
+                      const laser_b200_batch_strides *bs, const OperandOp *opA, const OperandOp *opB, const Epilogue &epi,
+                      int path, void *stream) {
+  if (batch < 0) return set_error(LASER_B200_EINVAL, "negative batch %lld", (long long)batch);
+  if (batch > 0 && !bs) return set_error(LASER_B200_EINVAL, "batchStrides is NULL");
+  if (batch > 1 && bs->C == 0) return set_error(LASER_B200_EINVAL, "batchStrides->C is 0: the problems' outputs would overlap");
+  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
+    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  int rc = check_args(M, N, K, A, B, C);
+  if (rc == -1 || batch == 0) return LASER_B200_OK;
+  if (rc) return rc;
+  if (batch == 1) return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, epi, nullptr, opA, opB);
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, K, epi, /*operand_op=*/true);
+  // chunks of whole problems: the prepared workspace stays under the cap, and the launch's tile counts -- batch x tiles x
+  // up to 16 K-splits -- fit in int32
+  const int64_t per = batch_ws_per_problem(path, M, N, K, !batch_shares(bs->A, opA, bs->auxA), !batch_shares(bs->B, opB, bs->auxB),
+                                           opA != nullptr, opB != nullptr);
+  int64_t chunk = per > 0 ? c->batch_ws_bytes / per : batch;
+  const int64_t tiles = ((M + TC_BLOCK_M - 1) / TC_BLOCK_M) * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N);
+  if (chunk > 0x7fffffffLL / (16 * tiles)) chunk = 0x7fffffffLL / (16 * tiles);
+  if (chunk < 1) chunk = 1;
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const BatchArgs bat{batch - b0 < chunk ? batch - b0 : chunk, bs->A, bs->B, bs->C, bs->auxA, bs->auxB};
+    OperandOp ca, cb;
+    if (opA) { ca = *opA; if (ca.aux) ca.aux += b0 * bs->auxA; }
+    if (opB) { cb = *opB; if (cb.aux) cb.aux += b0 * bs->auxB; }
+    if ((rc = batched_run(*c, path, bat, M, N, K, alpha, A + b0 * bs->A, rsA, csA, B + b0 * bs->B, rsB, csB, beta, C + b0 * bs->C, rsC,
+                          csC, s, epi, opA ? &ca : nullptr, opB ? &cb : nullptr)))
+      return rc;
+  }
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
+}
+// laser_b200_gemm_strided_batched_f32_fused_dev (defined with the other batched entries in capi_layers.inc)
+int batched_fused_entry(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
+                        const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
+                        const laser_b200_batch_strides *bs, const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
+                        const laser_b200_epilogue *epi, int path, void *stream) {
+  Epilogue e;
+  OperandOp oa, ob;
+  const OperandOp *pa, *pb;
+  int rc;
+  if ((rc = epilogue_of(epi, &e))) return rc;
+  if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
+  if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
+  return batched_fused_dev(batch, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, bs, pa, pb, e, path, stream);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1550,5 +1721,6 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 
 }  // extern "C"
 
+#define LB200_BATCHED_FUSED_F32 batched_fused_entry
 #include "capi_layers.inc"
 #include "capi_multi.inc"

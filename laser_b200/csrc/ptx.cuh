@@ -85,6 +85,16 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *m
         "r"(c0), "r"(c1)
       : "memory");
 }
+// 3-D tiled load (box depth 1 along c2: one matrix of a batch; elements outside any extent are zero-filled)
+__device__ __forceinline__ void tma_load_3d(void *smem_dst, const CUtensorMap *map, uint64_t *bar,
+                                            int32_t c0, int32_t c1, int32_t c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)),
+        "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 // cp.async (LDGSTS): 8 bytes global -> shared without passing through registers; `valid` false: eight zero bytes instead
 __device__ __forceinline__ void cp_async_8(void *smem_dst, const void *gsrc, bool valid) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;"

@@ -96,20 +96,45 @@ __device__ __forceinline__ float4 op_vec(const OperandOp &op, float4 v, int64_t 
   return v;
 }
 
+// ---- batched preparation: the operands of bt.n problems in one launch ------------------------------------------------
+// The kernels below also take `template <bool BATCHED>` (false: one problem, `bt` never read).  A BATCHED kernel prepares bt.n
+// problems whose [R][Cc] views are bt.bs elements apart (aux: bt.aux_bs), and writes what one problem's launch writes,
+// stacked: pieces [bt.n * R][ld], per-row scale words [bt.n * R], per-column scale words [bt.n][Cc].
+struct Batch {
+  int64_t n = 1;
+  int64_t bs = 0, aux_bs = 0;
+};
+// stacked row g -> its problem's source (and aux) and the row within the problem
+template <bool BATCHED>
+__device__ __forceinline__ int64_t batch_row(int64_t g, int64_t R, const Batch &bt, const float *&src, OperandOp &op) {
+  if constexpr (BATCHED) {
+    const int64_t b = g / R;
+    src += b * bt.bs;
+    if (op.aux) op.aux += b * bt.aux_bs;
+    return g - b * R;
+  } else {
+    return g;
+  }
+}
+
 // src: R rows of Cc contiguous floats, leading dimension src_ld (16-byte aligned rows).
 // hi/lo: compact, leading dimension dst_ld (multiple of 4).
-template <bool HAS_OP = false>
+template <bool HAS_OP = false, bool BATCHED = false>
 __global__ void __launch_bounds__(256)
 split_rows_tf32_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld,
-                       float *__restrict__ hi, float *__restrict__ lo, int64_t dst_ld, OperandOp op = OperandOp()) {
+                       float *__restrict__ hi, float *__restrict__ lo, int64_t dst_ld, OperandOp op = OperandOp(),
+                       Batch bt = Batch()) {
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   const int64_t vec_per_row = (Cc + 3) >> 2;
-  const int64_t total = R * vec_per_row;
+  const int64_t total = (BATCHED ? bt.n * R : R) * vec_per_row;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int64_t r = i / vec_per_row;
     const int64_t c = (i - r * vec_per_row) << 2;
-    const float *s = src + r * src_ld + c;
+    const float *sp = src;
+    OperandOp o = op;
+    const int64_t rl = batch_row<BATCHED>(r, R, bt, sp, o);
+    const float *s = sp + rl * src_ld + c;
     float4 v;
     if (c + 4 <= Cc) {
       v = *reinterpret_cast<const float4 *>(s);
@@ -119,7 +144,8 @@ split_rows_tf32_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int
       v.z = (c + 2 < Cc) ? s[2] : 0.0f;
       v.w = 0.0f;
     }
-    if constexpr (HAS_OP) v = op_vec(op, v, r, c, Cc);
+    if constexpr (HAS_OP && BATCHED) v = op_vec(o, v, rl, c, Cc);
+    else if constexpr (HAS_OP) v = op_vec(op, v, r, c, Cc);
     float4 h, l;
     h.x = tf32_rna(v.x); l.x = tf32_lo(v.x, h.x);
     h.y = tf32_rna(v.y); l.y = tf32_lo(v.y, h.y);
@@ -142,11 +168,12 @@ __device__ __forceinline__ uint32_t finite_abs_bits(float f) {
 }
 constexpr int ABSMAX_ROW_CHUNK = 1024;   // floats of one row reduced by one warp pass (32 lanes x 8 x float4)
 constexpr int ABSMAX_COL_ROWS = 64;      // rows of a 4-column strip reduced by one thread
-template <bool PER_COL, bool HAS_OP = false>
+template <bool PER_COL, bool HAS_OP = false, bool BATCHED = false>
 __global__ void __launch_bounds__(256)
 absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld, uint32_t *__restrict__ out,
-                 OperandOp op = OperandOp()) {
+                 OperandOp op = OperandOp(), Batch bt = Batch()) {
   static_assert(PER_COL || !HAS_OP, "a K-major operand with an op takes the fused row kernel");
+  static_assert(PER_COL || !BATCHED, "a K-major operand takes the fused row kernel");
   if constexpr (!PER_COL) {
     // warp w takes (row, chunk) items; lanes read float4s 128 floats apart; butterfly max; one atomic per item
     const int lane = threadIdx.x & 31;
@@ -177,19 +204,29 @@ absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t s
     }
   } else {
     // thread takes (4-column strip, block of ABSMAX_COL_ROWS rows) items: adjacent threads read adjacent float4s
+    // (BATCHED: row blocks of one problem at a time, rb counting over the problems' blocks)
     const int64_t strips = (Cc + 3) >> 2;
     const int64_t rblocks = (R + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS;
-    const int64_t items = strips * rblocks;
+    const int64_t items = strips * (BATCHED ? bt.n * rblocks : rblocks);
     for (int64_t it = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; it < items;
          it += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-      const int64_t rb = it / strips;
+      int64_t rb = it / strips;
       const int64_t c = (it - rb * strips) << 2;
+      const float *src_b = src;
+      OperandOp o = op;
+      uint32_t *out_b = out;
+      if constexpr (BATCHED) {
+        const int64_t b = rb / rblocks;
+        rb -= b * rblocks;
+        batch_row<true>(b * R, R, bt, src_b, o);
+        out_b += b * Cc;
+      }
       const int64_t r1 = (rb + 1) * ABSMAX_COL_ROWS < R ? (rb + 1) * ABSMAX_COL_ROWS : R;
       uint32_t m0 = 0u, m1 = 0u, m2 = 0u, m3 = 0u;
       for (int64_t r = rb * ABSMAX_COL_ROWS; r < r1; ++r) {
-        const float *s = src + r * src_ld + c;
+        const float *s = src_b + r * src_ld + c;
         if constexpr (HAS_OP) {   // the scale is taken over the op's output (padding lanes are 0)
-          const float4 v = op_vec(op, load_row_vec(src + r * src_ld, c, Cc), r, c, Cc);
+          const float4 v = op_vec(BATCHED ? o : op, load_row_vec(src_b + r * src_ld, c, Cc), r, c, Cc);
           m0 = max(m0, finite_abs_bits(v.x)); m1 = max(m1, finite_abs_bits(v.y));
           m2 = max(m2, finite_abs_bits(v.z)); m3 = max(m3, finite_abs_bits(v.w));
         } else if (c + 4 <= Cc) {
@@ -202,10 +239,10 @@ absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t s
           if (c + 2 < Cc) m2 = max(m2, finite_abs_bits(s[2]));
         }
       }
-      atomicMax(out + c, m0);
-      if (c + 1 < Cc) atomicMax(out + c + 1, m1);
-      if (c + 2 < Cc) atomicMax(out + c + 2, m2);
-      if (c + 3 < Cc) atomicMax(out + c + 3, m3);
+      atomicMax(out_b + c, m0);
+      if (c + 1 < Cc) atomicMax(out_b + c + 1, m1);
+      if (c + 2 < Cc) atomicMax(out_b + c + 2, m2);
+      if (c + 3 < Cc) atomicMax(out_b + c + 3, m3);
     }
   }
 }
@@ -227,10 +264,11 @@ __device__ __forceinline__ void store_f16x2_vec(float4 v, float s, uint16_t *hro
 // thread; what is left of a longer row is read twice, the second time from L2), reduces the abs-max, writes the word and
 // both fp16 pieces: 4 bytes read + 4 written per element, against 8 + 4 for abs-max and split as two kernels.
 constexpr int F16ROWS_MAXV = 8;
-template <int GROUP, bool HAS_OP = false>
+template <int GROUP, bool HAS_OP = false, bool BATCHED = false>
 __global__ void __launch_bounds__(256, 4)
 f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *__restrict__ hb,
-                        uint16_t *__restrict__ lb, int64_t ld_b, uint32_t *__restrict__ absmax, OperandOp op = OperandOp()) {
+                        uint16_t *__restrict__ lb, int64_t ld_b, uint32_t *__restrict__ absmax, OperandOp op = OperandOp(),
+                        Batch bt = Batch()) {
   static_assert(GROUP == 32 || GROUP == 256, "a warp or the CTA per row");
   __shared__ uint32_t red[2][8];
   ptx::griddep_launch_dependents();
@@ -241,8 +279,12 @@ f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
   const int64_t nvec = (Cc + 3) >> 2;
   int parity = 0;
   // GROUP == 256: every thread of the CTA runs the same number of iterations (the loop holds a __syncthreads)
-  for (int64_t r = first; r < R; r += step) {
-    const float *row = src + r * src_ld;
+  const int64_t rows = BATCHED ? bt.n * R : R;
+  for (int64_t r = first; r < rows; r += step) {
+    const float *sp = src;
+    OperandOp o = op;
+    const int64_t rl = batch_row<BATCHED>(r, R, bt, sp, o);
+    const float *row = sp + rl * src_ld;
     float4 v[F16ROWS_MAXV];
     uint32_t m = 0u;
 #pragma unroll
@@ -250,13 +292,13 @@ f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
       const int64_t idx = tid + static_cast<int64_t>(i) * GROUP;
       if (idx < nvec) {
         v[i] = load_row_vec(row, idx << 2, Cc);
-        if constexpr (HAS_OP) v[i] = op_vec(op, v[i], r, idx << 2, Cc);
+        if constexpr (HAS_OP) v[i] = op_vec(o, v[i], rl, idx << 2, Cc);
         m = max(max(m, finite_abs_bits(v[i].x)), max(finite_abs_bits(v[i].y), max(finite_abs_bits(v[i].z), finite_abs_bits(v[i].w))));
       }
     }
     for (int64_t idx = tid + static_cast<int64_t>(F16ROWS_MAXV) * GROUP; idx < nvec; idx += GROUP) {
       float4 t = load_row_vec(row, idx << 2, Cc);
-      if constexpr (HAS_OP) t = op_vec(op, t, r, idx << 2, Cc);
+      if constexpr (HAS_OP) t = op_vec(o, t, rl, idx << 2, Cc);
       m = max(max(m, finite_abs_bits(t.x)), max(finite_abs_bits(t.y), max(finite_abs_bits(t.z), finite_abs_bits(t.w))));
     }
     float mf = __uint_as_float(m);     // non-negative finite: fmaxf orders them like the integers
@@ -279,7 +321,7 @@ f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
       if (idx < nvec) store_f16x2_vec(v[i], s, hrow, lrow, idx << 2);
     }
     for (int64_t idx = tid + static_cast<int64_t>(F16ROWS_MAXV) * GROUP; idx < nvec; idx += GROUP) {
-      if constexpr (HAS_OP) store_f16x2_vec(op_vec(op, load_row_vec(row, idx << 2, Cc), r, idx << 2, Cc), s, hrow, lrow, idx << 2);
+      if constexpr (HAS_OP) store_f16x2_vec(op_vec(o, load_row_vec(row, idx << 2, Cc), rl, idx << 2, Cc), s, hrow, lrow, idx << 2);
       else store_f16x2_vec(load_row_vec(row, idx << 2, Cc), s, hrow, lrow, idx << 2);
     }
   }
@@ -371,33 +413,47 @@ inline bool f16x2_rows_ring_ok(const float *src, int64_t Cc, int64_t src_ld) {
 // SPLIT_ROWS rows): a thread owns 4 columns of the strip -- for PER_COL their four scales are computed once -- and walks
 // the rows of the block, adjacent threads reading adjacent float4s.
 constexpr int SPLIT_ROWS = 64;
-template <bool PER_COL, bool HAS_OP = false>
+template <bool PER_COL, bool HAS_OP = false, bool BATCHED = false>
 __global__ void __launch_bounds__(256)
 split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld,
                         uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld_b,
-                        const uint32_t *__restrict__ absmax, OperandOp op = OperandOp()) {
+                        const uint32_t *__restrict__ absmax, OperandOp op = OperandOp(), Batch bt = Batch()) {
+  static_assert(PER_COL || !BATCHED, "a K-major operand takes the fused row kernel");
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   const int tx = static_cast<int>(threadIdx.x) & 63, ty = static_cast<int>(threadIdx.x) >> 6;   // 64 float4 columns x 4 row lanes
   const int64_t strips = (Cc + 255) >> 8;
   const int64_t rblocks = (R + SPLIT_ROWS - 1) / SPLIT_ROWS;
-  for (int64_t it = blockIdx.x; it < strips * rblocks; it += gridDim.x) {
-    const int64_t rb = it / strips;
+  for (int64_t it = blockIdx.x; it < strips * (BATCHED ? bt.n * rblocks : rblocks); it += gridDim.x) {
+    int64_t rb = it / strips;
     const int64_t c = ((it - rb * strips) << 8) + (tx << 2);
     if (c >= Cc) continue;
+    // (BATCHED: row block rb of problem b; its pieces are rows b * R + r of hb / lb, its words absmax[b * Cc ..])
+    const float *src_b = src;
+    OperandOp o = op;
+    const uint32_t *absmax_b = absmax;
+    uint16_t *hb_b = hb, *lb_b = lb;
+    if constexpr (BATCHED) {
+      const int64_t b = rb / rblocks;
+      rb -= b * rblocks;
+      batch_row<true>(b * R, R, bt, src_b, o);
+      absmax_b += b * Cc;
+      hb_b += b * R * ld_b;
+      lb_b += b * R * ld_b;
+    }
     float sx = 1.0f, sy = 1.0f, sz = 1.0f, sw = 1.0f;
     if constexpr (PER_COL) {
-      sx = f16x2_scale(absmax[c]);
-      sy = (c + 1 < Cc) ? f16x2_scale(absmax[c + 1]) : 1.0f;
-      sz = (c + 2 < Cc) ? f16x2_scale(absmax[c + 2]) : 1.0f;
-      sw = (c + 3 < Cc) ? f16x2_scale(absmax[c + 3]) : 1.0f;
+      sx = f16x2_scale(absmax_b[c]);
+      sy = (c + 1 < Cc) ? f16x2_scale(absmax_b[c + 1]) : 1.0f;
+      sz = (c + 2 < Cc) ? f16x2_scale(absmax_b[c + 2]) : 1.0f;
+      sw = (c + 3 < Cc) ? f16x2_scale(absmax_b[c + 3]) : 1.0f;
     }
     const int64_t r1 = (rb + 1) * SPLIT_ROWS < R ? (rb + 1) * SPLIT_ROWS : R;
 #pragma unroll 4
     for (int64_t r = rb * SPLIT_ROWS + ty; r < r1; r += 4) {
-      float4 v = load_row_vec(src + r * src_ld, c, Cc);
-      if constexpr (HAS_OP) v = op_vec(op, v, r, c, Cc);
-      if constexpr (!PER_COL) sx = sy = sz = sw = f16x2_scale(absmax[r]);
-      store_f16x2_vec4(v, sx, sy, sz, sw, hb + r * ld_b, lb + r * ld_b, c);
+      float4 v = load_row_vec(src_b + r * src_ld, c, Cc);
+      if constexpr (HAS_OP) v = op_vec(o, v, r, c, Cc);
+      if constexpr (!PER_COL) sx = sy = sz = sw = f16x2_scale(absmax_b[r]);
+      store_f16x2_vec4(v, sx, sy, sz, sw, hb_b + r * ld_b, lb_b + r * ld_b, c);
     }
   }
 }
@@ -407,27 +463,41 @@ split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
 // store (along c) are coalesced.  SPLIT: also write lo (fp32 only).
 // MODE 0: plain copy; 1: fp32 hi/lo pieces (dst, dst_lo).
 // HAS_OP (fp32): the op is applied to each element as it is gathered (aux read with its own strides).
-template <typename T, int MODE, bool HAS_OP = false>
+template <typename T, int MODE, bool HAS_OP = false, bool BATCHED = false>
 __global__ void __launch_bounds__(256)
 pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr, int64_t sc,
-                    T *__restrict__ dst, T *__restrict__ dst_lo, int64_t ld, int read_along_r, OperandOp op = OperandOp()) {
+                    T *__restrict__ dst, T *__restrict__ dst_lo, int64_t ld, int read_along_r, OperandOp op = OperandOp(),
+                    Batch bt = Batch()) {
   static_assert(!HAS_OP || sizeof(T) == 4, "operand ops are fp32 only");
+  static_assert(!BATCHED || sizeof(T) == 4, "batched operands are fp32 only");
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   __shared__ T tile[32][33];
   const int64_t tiles_c = (Cc + 31) >> 5;
   const int64_t tiles_r = (R + 31) >> 5;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
-  for (int64_t t = blockIdx.x; t < tiles_r * tiles_c; t += gridDim.x) {
-    const int64_t r0 = (t / tiles_c) << 5, c0 = (t % tiles_c) << 5;
+  for (int64_t t = blockIdx.x; t < tiles_r * tiles_c * (BATCHED ? bt.n : 1); t += gridDim.x) {
+    int64_t r0 = (t / tiles_c) << 5;
+    const int64_t c0 = (t % tiles_c) << 5;
+    const T *src_t = src;
+    T *dst_t = dst, *dlo_t = dst_lo;
+    OperandOp o = op;
+    if constexpr (BATCHED) {   // a tile of problem b: read from its operand and aux, written to rows b * R + r of dst
+      const int64_t b = (t / tiles_c) / tiles_r;
+      r0 -= (b * tiles_r) << 5;
+      src_t += b * bt.bs;
+      if (o.aux) o.aux += b * bt.aux_bs;
+      dst_t += b * R * ld;
+      if constexpr (MODE == 1) dlo_t += b * R * ld;
+    }
     if (read_along_r) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int64_t c = c0 + ty + i * 8, r = r0 + tx;
         if constexpr (HAS_OP) {
           if (r < R && c < Cc)
-            tile[tx][ty + i * 8] = operand_op(op.op, src[r * sr + c * sc], op.aux ? op.aux[r * op.aux_sr + c * op.aux_sc] : 0.0f);
+            tile[tx][ty + i * 8] = operand_op(o.op, src_t[r * sr + c * sc], o.aux ? o.aux[r * o.aux_sr + c * o.aux_sc] : 0.0f);
         } else {
-          if (r < R && c < Cc) tile[tx][ty + i * 8] = src[r * sr + c * sc];
+          if (r < R && c < Cc) tile[tx][ty + i * 8] = src_t[r * sr + c * sc];
         }
       }
     } else {
@@ -436,9 +506,9 @@ pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr
         const int64_t r = r0 + ty + i * 8, c = c0 + tx;
         if constexpr (HAS_OP) {
           if (r < R && c < Cc)
-            tile[ty + i * 8][tx] = operand_op(op.op, src[r * sr + c * sc], op.aux ? op.aux[r * op.aux_sr + c * op.aux_sc] : 0.0f);
+            tile[ty + i * 8][tx] = operand_op(o.op, src_t[r * sr + c * sc], o.aux ? o.aux[r * o.aux_sr + c * o.aux_sc] : 0.0f);
         } else {
-          if (r < R && c < Cc) tile[ty + i * 8][tx] = src[r * sr + c * sc];
+          if (r < R && c < Cc) tile[ty + i * 8][tx] = src_t[r * sr + c * sc];
         }
       }
     }
@@ -450,10 +520,10 @@ pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr
         const T v = tile[ty + i * 8][tx];
         if constexpr (MODE == 1) {
           const float h = tf32_rna(v);
-          dst[r * ld + c] = h;
-          dst_lo[r * ld + c] = tf32_lo(v, h);
+          dst_t[r * ld + c] = h;
+          dlo_t[r * ld + c] = tf32_lo(v, h);
         } else {
-          dst[r * ld + c] = v;
+          dst_t[r * ld + c] = v;
         }
       }
     }
@@ -463,11 +533,13 @@ pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr
 
 // Second half of a split-K GEMM (tc_params.h): C <- act(alpha * sum_s ws[s][i] + beta * C + bias) over the split tiles
 // n_direct + i, i < n_tail, planes added in the fixed order s = 0 .. S-1 (deterministic).  ws: [S][n_tail][tile_m][TC_BLOCK_N]
-// fp32, tile-local.  Item = four consecutive columns of one tile row.
+// fp32, tile-local.  Item = four consecutive columns of one tile row.  BATCHED: tile t of the launch is tile t % (num_m * num_n)
+// of problem t / (num_m * num_n), whose C starts bsC elements after the previous problem's (tc_params.h).
+template <bool BATCHED = false>
 __global__ void __launch_bounds__(256)
 splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n_direct, int num_m, int num_n, int raster_g,
                           int tile_m, int64_t M, int64_t N, float alpha, float beta, float *__restrict__ C, int64_t rsC,
-                          int64_t csC, const float *__restrict__ bias, int bias_per_row, int act) {
+                          int64_t csC, const float *__restrict__ bias, int bias_per_row, int act, int64_t bsC = 0) {
   constexpr int V = TC_BLOCK_N / 4;   // float4 per tile row
   const int64_t per_tile = static_cast<int64_t>(tile_m) * V;
   const int64_t total = static_cast<int64_t>(n_tail) * per_tile;
@@ -477,8 +549,14 @@ splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n
     const int ti = static_cast<int>(i / per_tile);
     const int64_t rem = i - ti * per_tile;
     const int r_l = static_cast<int>(rem / V), c4 = static_cast<int>(rem - static_cast<int64_t>(r_l) * V);
-    int mb, nb;
-    tile_coords(n_direct + ti, num_m, num_n, raster_g, mb, nb);
+    int mb, nb, t = n_direct + ti;
+    float *Cb = C;
+    if constexpr (BATCHED) {
+      const int b = t / (num_m * num_n);
+      t -= b * (num_m * num_n);
+      Cb += b * bsC;
+    }
+    tile_coords(t, num_m, num_n, raster_g, mb, nb);
     const int64_t r = static_cast<int64_t>(mb) * tile_m + r_l, c = static_cast<int64_t>(nb) * TC_BLOCK_N + 4 * c4;
     if (r >= M || c >= N) continue;
     const float *src = ws + i * 4;
@@ -488,7 +566,7 @@ splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n
       sum.x = __fadd_rn(sum.x, t.x); sum.y = __fadd_rn(sum.y, t.y); sum.z = __fadd_rn(sum.z, t.z); sum.w = __fadd_rn(sum.w, t.w);
     }
     const float sv[4] = {sum.x, sum.y, sum.z, sum.w};
-    float *dst = C + r * rsC + c * csC;
+    float *dst = Cb + r * rsC + c * csC;
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       if (c + e < N) {

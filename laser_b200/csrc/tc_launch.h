@@ -14,6 +14,7 @@ struct TcLaunch {
   TcParams p;
   bool a_mn = false, b_mn = false;   // operand major-ness
   bool pair = false;                 // clusters of two CTAs sharing one tile scheduler
+  bool batched = false;              // p.batch problems, rank-3 tensor maps (fp32 families, single CTAs: tc_params.h)
   bool pdl = false;                  // programmatic dependent launch: overlap the prologue with the preceding kernel's tail
   int dev = 0, sm_count = 0;
   cudaStream_t stream = nullptr;

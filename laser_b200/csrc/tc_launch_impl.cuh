@@ -13,7 +13,7 @@
 
 namespace lb200 {
 
-template <int ESZ, uint32_t FMT16, int NPASS, typename OutT, bool SCALED, bool PAIR, bool A_MN, bool B_MN>
+template <int ESZ, uint32_t FMT16, int NPASS, typename OutT, bool SCALED, bool PAIR, bool A_MN, bool B_MN, bool BATCHED = false>
 int launch_tc_one(const TcLaunch &l) {
   using Cfg = TcCfg<NPASS, PAIR>;
   const int64_t units_total = tc_units(l.p);  // work units
@@ -37,7 +37,10 @@ int launch_tc_one(const TcLaunch &l) {
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 2;
   }
-  auto kfn = gemm_tc_kernel<ESZ, FMT16, NPASS, A_MN, B_MN, OutT, PAIR, SCALED>;
+  auto kfn = [] {
+    if constexpr (BATCHED) return gemm_tc_batched_kernel<ESZ, FMT16, NPASS, A_MN, B_MN, OutT, SCALED>;
+    else return gemm_tc_kernel<ESZ, FMT16, NPASS, A_MN, B_MN, OutT, PAIR, SCALED>;
+  }();
   static std::atomic<uint32_t> attr_set{0};   // per device: function attributes live in the context
   if (!(attr_set.load(std::memory_order_acquire) & (1u << l.dev))) {
     const cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -51,19 +54,25 @@ template <int ESZ, uint32_t FMT16, int NPASS, typename OutT, bool SCALED>
 int launch_tc_family(const TcLaunch &l) {
   if constexpr (ESZ == 4) {   // wgmma reads tf32 tiles K-major only: capi.cu prepares MN-major fp32 operands K-major
     if (l.a_mn || l.b_mn) return static_cast<int>(cudaErrorNotSupported);
+    if (l.batched) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, false, false, false, true>(l);
     if (l.pair) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, true, false, false>(l);
     return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, false, false, false>(l);
   }
-#define LB200_MAJORS(PAIR)                                                                                   \
-  do {                                                                                                       \
-    if (!l.a_mn && !l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, false, false>(l);    \
-    if (!l.a_mn && l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, false, true>(l);      \
-    if (l.a_mn && !l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, true, false>(l);      \
-    return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, true, true>(l);                              \
+#define LB200_MAJORS(PAIR, BATCHED)                                                                                   \
+  do {                                                                                                                \
+    if (!l.a_mn && !l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, false, false, BATCHED>(l);    \
+    if (!l.a_mn && l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, false, true, BATCHED>(l);      \
+    if (l.a_mn && !l.b_mn) return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, true, false, BATCHED>(l);      \
+    return launch_tc_one<ESZ, FMT16, NPASS, OutT, SCALED, PAIR, true, true, BATCHED>(l);                              \
   } while (0)
   if constexpr (ESZ == 2) {
-    if (l.pair) LB200_MAJORS(true);
-    LB200_MAJORS(false);
+    // batched: the fp32 families only (F16X3 here; bf16 has no batched entry)
+    if constexpr (SCALED) {
+      if (l.batched) LB200_MAJORS(false, true);
+    }
+    if (l.batched) return static_cast<int>(cudaErrorNotSupported);
+    if (l.pair) LB200_MAJORS(true, false);
+    LB200_MAJORS(false, false);
   }
 #undef LB200_MAJORS
 }

@@ -69,6 +69,14 @@ struct TcParams {
   // tile scheduler: word 0 = next unit (atomicAdd), word 1 = pairs that have drawn their last unit (the last one zeroes
   // both words for the next launch that uses this slot).  nullptr: static round-robin (unit = pair index + i * pairs)
   unsigned int *sched = nullptr;
+  // batched launch (gemm_tc_kernel<..., BATCHED = true>): `batch` problems of M x N x K.  Tile t of the launch is tile
+  // t % (num_m_blocks * num_n_blocks) of problem t / (num_m_blocks * num_n_blocks); split-K and the raster order apply to
+  // these tiles as above.  Problem b reads slice b * map_b_a (b * map_b_b) of A's (B's) rank-3 tensor maps -- 0 for an
+  // operand the batch shares --, writes C + b * bsC and reads its scale words b * amax_bs_a (b * amax_bs_b) further on.
+  int batch = 1;
+  int map_b_a = 0, map_b_b = 0;
+  int64_t bsC = 0;
+  int64_t amax_bs_a = 0, amax_bs_b = 0;
 };
 
 // raster order of the output tiles: groups of G m-blocks sweep n together, so that the concurrently resident tiles (132 of
@@ -111,7 +119,7 @@ inline void tc_plan(TcParams &p, int npass, bool pair, const TcPlanCfg &cfg) {
   p.num_m_blocks = static_cast<int>((p.M + tile_m - 1) / tile_m);
   p.num_n_blocks = static_cast<int>((p.N + TC_BLOCK_N - 1) / TC_BLOCK_N);
   // ---- split-K (fp32 output only): too few output tiles to fill the machine and a long K, or a thin last wave ----
-  const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks;
+  const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks * p.batch;
   p.k_splits = 1;
   p.kb_per_split = num_kb;
   p.n_direct = static_cast<int>(tiles);
@@ -141,11 +149,11 @@ inline void tc_plan(TcParams &p, int npass, bool pair, const TcPlanCfg &cfg) {
 }
 // work units of a planned launch, and the fp32 words of its split-K workspace (0: nothing is split)
 inline int64_t tc_units(const TcParams &p) {
-  const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks;
+  const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks * p.batch;
   return p.n_direct + (tiles - p.n_direct) * p.k_splits;
 }
 inline int64_t tc_split_ws_floats(const TcParams &p, bool pair) {
-  const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks;
+  const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks * p.batch;
   const int64_t tile_m = pair ? 2 * TC_BLOCK_M : TC_BLOCK_M;
   return (tiles - p.n_direct) * p.k_splits * tile_m * TC_BLOCK_N;
 }

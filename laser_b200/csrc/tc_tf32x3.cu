@@ -1,4 +1,5 @@
-// tc_tf32x3.cu -- the two instantiations (K-major operands x single CTA / cluster of two) of gemm_tc_kernel<4, ptx::kFmtBF16, 3, float, false>
+// tc_tf32x3.cu -- the two instantiations (K-major operands x single CTA / cluster of two) of gemm_tc_kernel<4, ptx::kFmtBF16, 3, float, false>,
+// and gemm_tc_batched_kernel
 #include "tc_launch_impl.cuh"
 
 namespace lb200 {

@@ -21,7 +21,7 @@ from . import _capi
 from ._capi import (PATH_AUTO, PATH_BF16, PATH_F16X3, PATH_SIMT, PATH_TF32X1, PATH_TF32X3,
                     LaserB200Error, check, lib)
 
-__all__ = ["gemm_strided", "gemm_strided_fused", "DevPtr", "last_path", "launch_count", "set_f32_mode", "get_f32_mode",
+__all__ = ["gemm_strided", "gemm_strided_fused", "gemm_strided_batched_fused", "DevPtr", "last_path", "launch_count", "set_f32_mode", "get_f32_mode",
            "fill_uniform_f32", "init", "shutdown", "synchronize", "profile_begin", "profile_end"]
 
 _NP_DTYPES = {np.dtype(np.float32): "f32", np.dtype(np.float64): "f64", np.dtype(np.int32): "i32",
@@ -137,24 +137,29 @@ def gemm_strided(M, N, K, alpha, A, rowStrideA, colStrideA, B, rowStrideB, colSt
         check(getattr(L, "laser_b200_gemm_strided_%s_dev" % ta)(*args, stream))
 
 
-def _operand_op(spec):
-    """op_a / op_b of gemm_strided_fused -> an OperandOp, or None"""
+def _operand_op(spec, batched=False):
+    """op_a / op_b of gemm_strided_fused -> (an OperandOp or None, aux batch stride).  batched: the aux tensor also takes its
+    batch stride, (name, aux, auxRowStride, auxColStride, auxBatchStride)."""
     if spec is None:
-        return None
+        return None, 0
     if isinstance(spec, str):
         spec = (spec,)
     name, rest = spec[0], tuple(spec[1:])
     op = _capi.OperandOp()
     op.op = _capi.OP_NAMES[name]
+    aux_bs = 0
     if rest:
-        if len(rest) != 3:
-            raise ValueError("an operand op is a name or (name, aux, auxRowStride, auxColStride)")
+        if len(rest) != (4 if batched else 3):
+            raise ValueError("an operand op is a name or (name, aux, auxRowStride, auxColStride%s)" %
+                             (", auxBatchStride" if batched else ""))
         paux, taux, daux = _resolve(rest[0])
         if not daux or taux != "f32":
             raise TypeError("aux must be a float32 device buffer")
         op.aux = paux
         op.auxRowStride, op.auxColStride = int(rest[1]), int(rest[2])
-    return op
+        if batched:
+            aux_bs = int(rest[3])
+    return op, aux_bs
 
 
 def gemm_strided_fused(M, N, K, alpha, A, rowStrideA, colStrideA, B, rowStrideB, colStrideB, beta, C,
@@ -166,18 +171,8 @@ def gemm_strided_fused(M, N, K, alpha, A, rowStrideA, colStrideA, B, rowStrideB,
     "relu", "tanh", "sigmoid", or a derivative with its aux tensor and that tensor's element strides,
     e.g. op_a=("relu_grad", Z, rowStrideZ, colStrideZ) for dY * relu'(Z); also "tanh_grad" (aux: the
     tanh output) and "sigmoid_grad" (aux: the sigmoid output)."""
-    pa, ta, da = _resolve(A); pb, tb, db = _resolve(B); pc, tc, dc = _resolve(C)
-    if not (ta == tb == tc == "f32") or not (da and db and dc):
-        raise TypeError("gemm_strided_fused takes float32 device buffers")
-    epi = _capi.Epilogue()
-    if bias is not None:
-        pbias, tbias, dbias = _resolve(bias)
-        if not dbias or tbias != "f32":
-            raise TypeError("bias must be a float32 device vector")
-        epi.bias = pbias
-    epi.bias_per_row = 1 if bias_per_row else 0
-    epi.activation = {"none": 0, "relu": 1, "tanh": 2, "sigmoid": 3}[activation]
-    oa, ob = _operand_op(op_a), _operand_op(op_b)
+    pa, pb, pc, epi = _fused_args("gemm_strided_fused", A, B, C, bias, bias_per_row, activation)
+    (oa, _), (ob, _) = _operand_op(op_a), _operand_op(op_b)
     if stream is None:
         stream = _current_stream()
     if oa is None and ob is None:
@@ -190,6 +185,40 @@ def gemm_strided_fused(M, N, K, alpha, A, rowStrideA, colStrideA, B, rowStrideB,
                                                       ctypes.byref(oa) if oa is not None else None,
                                                       ctypes.byref(ob) if ob is not None else None,
                                                       ctypes.byref(epi), path, stream))
+
+
+def _fused_args(fn, A, B, C, bias, bias_per_row, activation):
+    """-> (A, B, C addresses, Epilogue) of a fused entry"""
+    pa, ta, da = _resolve(A); pb, tb, db = _resolve(B); pc, tc, dc = _resolve(C)
+    if not (ta == tb == tc == "f32") or not (da and db and dc):
+        raise TypeError("%s takes float32 device buffers" % fn)
+    epi = _capi.Epilogue()
+    if bias is not None:
+        pbias, tbias, dbias = _resolve(bias)
+        if not dbias or tbias != "f32":
+            raise TypeError("bias must be a float32 device vector")
+        epi.bias = pbias
+    epi.bias_per_row = 1 if bias_per_row else 0
+    epi.activation = {"none": 0, "relu": 1, "tanh": 2, "sigmoid": 3}[activation]
+    return pa, pb, pc, epi
+
+
+def gemm_strided_batched_fused(batch, M, N, K, alpha, A, rowStrideA, colStrideA, batchStrideA, B, rowStrideB, colStrideB,
+                               batchStrideB, beta, C, rowStrideC, colStrideC, batchStrideC, bias=None, bias_per_row=False,
+                               activation="none", path=PATH_AUTO, stream=None, *, op_a=None, op_b=None):
+    """gemm_strided_fused over a batch on float32 DEVICE buffers: problem b reads A + b * batchStrideA, B + b * batchStrideB
+    and writes C + b * batchStrideC (a batch stride of 0 shares A or B; the bias is shared).  Every problem's operands are
+    prepared together and one GEMM launch runs the tiles of all of them.  op_a / op_b as in gemm_strided_fused, with the aux
+    tensor's batch stride last: e.g. op_a=("relu_grad", Z, rowStrideZ, colStrideZ, batchStrideZ)."""
+    pa, pb, pc, epi = _fused_args("gemm_strided_batched_fused", A, B, C, bias, bias_per_row, activation)
+    (oa, aux_a), (ob, aux_b) = _operand_op(op_a, batched=True), _operand_op(op_b, batched=True)
+    strides = _capi.BatchStrides(int(batchStrideA), int(batchStrideB), int(batchStrideC), aux_a, aux_b)
+    if stream is None:
+        stream = _current_stream()
+    check(lib().laser_b200_gemm_strided_batched_f32_fused_dev(
+        int(batch), M, N, K, float(alpha), pa, rowStrideA, colStrideA, pb, rowStrideB, colStrideB, float(beta), pc, rowStrideC,
+        colStrideC, ctypes.byref(strides), ctypes.byref(oa) if oa is not None else None,
+        ctypes.byref(ob) if ob is not None else None, ctypes.byref(epi), path, stream))
 
 
 def last_path():

@@ -35,6 +35,10 @@ type
     aux*: ptr float32                          # device; the derivative ops only
     auxRowStride*, auxColStride*: int64
 
+  LaserB200BatchStrides* {.bycopy.} = object   # laser_b200_batch_strides: element offsets between consecutive problems
+    A*, B*, C*: int64                          # 0 shares A (or B) across the batch; C may not be shared
+    auxA*, auxB*: int64                        # the same for the aux tensors of opA / opB
+
 {.push importc, cdecl, dynlib: laserB200Lib.}
 proc laser_b200_init*(): cint
 proc laser_b200_shutdown*()
@@ -109,6 +113,13 @@ proc laser_b200_gemm_strided_f32_fused_dev*(M, N, K: int64, alpha: float32,
     A: ptr float32, rowStrideA, colStrideA: int64,
     B: ptr float32, rowStrideB, colStrideB: int64,
     beta: float32, C: ptr float32, rowStrideC, colStrideC: int64,
+    opA, opB: ptr LaserB200OperandOp, epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
+# batched fused product (README.md:253-263): problem b reads X + b * batchStrides.X; one GEMM launch for the whole batch
+proc laser_b200_gemm_strided_batched_f32_fused_dev*(batch, M, N, K: int64, alpha: float32,
+    A: ptr float32, rowStrideA, colStrideA: int64,
+    B: ptr float32, rowStrideB, colStrideB: int64,
+    beta: float32, C: ptr float32, rowStrideC, colStrideC: int64,
+    batchStrides: ptr LaserB200BatchStrides,
     opA, opB: ptr LaserB200OperandOp, epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
 proc laser_b200_malloc*(devPtr: ptr pointer, bytes: csize_t): cint
 proc laser_b200_free*(devPtr: pointer): cint
