@@ -218,9 +218,8 @@ int laser_b200_gemm_strided_f32_fused_dev(int64_t M, int64_t N, int64_t K, float
  *   launched and C is untouched.
  *   LASER_B200_EINVAL, before anything is launched: batch < 0; batchStrides == NULL with batch > 0; batchStrides->C == 0 with
  *   batch > 1; an unknown op, or a derivative op without aux; an unknown path.
- *   LASER_B200_CTA_PAIR does not apply: batched launches use single CTAs.  A batch whose prepared operands would exceed
- *   LASER_B200_BATCH_WS_MB megabytes (read at initialisation, default 1024) runs in chunks of whole problems, one preparation
- *   and one GEMM launch sequence per chunk. */
+ *   A batch whose prepared operands would exceed LASER_B200_BATCH_WS_MB megabytes (read at initialisation, default 1024)
+ *   runs in chunks of whole problems, one preparation and one GEMM launch sequence per chunk. */
 typedef struct {
   int64_t A, B, C;    /* element offset between consecutive problems; 0 shares A (or B) across the batch */
   int64_t auxA, auxB; /* the same for opA->aux / opB->aux (ignored without a derivative op) */

@@ -106,10 +106,6 @@ struct Ctx {
   bool ring_attr_set = false, dmma_attr_set = false;
   int64_t panel_rows = 1024;  // env LASER_B200_PANEL_ROWS: row-panel height of the pipelined host-pointer entry
   bool panel_taper = false;   // env LASER_B200_PANEL_TAPER=1: cut the last row panel finer (shorter PCIe tail)
-  // env LASER_B200_CTA_PAIR=1: clusters of two CTAs on neighbouring 128-row blocks of one B panel, sharing one tile
-  // scheduler.  Off by default: each CTA still loads its own B tile, and in alternated runs at 8192^3 the pairing was 3-4 %
-  // faster on an H100 SXM at 700 W but 5 % slower on one at 400 W
-  bool cta_pair = false;
   // K extent per accumulator block of the fp32-faithful modes (env LASER_B200_KC): the tensor core's own accumulation does
   // not round to nearest, and its bias grows with the chain it accumulates; after each block the sums are added to fp32
   // running sums with round-to-nearest.  Shorter blocks cost a few register additions per k-tile.
@@ -134,7 +130,7 @@ struct Ctx {
   Buffer layer_ws;   // im2col workspace of the host-pointer convolution
   Buffer f16s;       // F16X3 mode: fp32 bits of max_k |a| per row of A (words [0, M)) and of max_k |b| per column of B (from
                      // f16_b_off on), written and read on the device
-  Buffer sched;      // kSchedSlots x {next unit, pairs done}: the kernel re-zeroes its slot when it ends
+  Buffer sched;      // kSchedSlots x {next unit, CTAs done}: the kernel re-zeroes its slot when it ends
   int sched_next = 0;
   cudaEvent_t ws_free = nullptr;  // recorded after the last kernel that reads ws[]
   std::mutex mu;       // workspace + tensor-map construction
@@ -192,7 +188,6 @@ int get_ctx(Ctx **out) {
         const int v = atoi(kc);
         if (v >= 32) c.kc_faithful = v;
       }
-      if (const char *cp = getenv("LASER_B200_CTA_PAIR")) c.cta_pair = atoi(cp) != 0;
       if (const char *rg = getenv("LASER_B200_RASTER")) c.raster_g = atoi(rg);
       if (const char *sk = getenv("LASER_B200_SPLITK")) c.splitk_enabled = atoi(sk) != 0;
       if (const char *dm = getenv("LASER_B200_F64_DMMA")) c.f64_dmma = atoi(dm) != 0;
@@ -204,7 +199,7 @@ int get_ctx(Ctx **out) {
         if (v >= 1) c.batch_ws_bytes = v << 20;
       }
       if (const char *pr = getenv("LASER_B200_PANEL_ROWS")) {
-        const int64_t v = atoll(pr) / 256 * 256;   // whole CTA-pair tiles
+        const int64_t v = atoll(pr) / 256 * 256;   // whole multiples of 256 rows, as the option has always been read
         if (v >= 256) c.panel_rows = v;
       }
       if (g_f32_mode.load() < 0) g_f32_mode.store(parse_f32_mode(getenv("LASER_B200_F32_MODE")));
@@ -668,21 +663,20 @@ struct BatchArgs {
 };
 
 // launch the tensor-core kernel on prepared operands (c.mu held by the caller).  bat: a batched launch (tc_params.h; the maps
-// are rank 3, single CTAs), with a_shared / b_shared for operands prepared once for the whole batch.
+// are rank 3), with a_shared / b_shared for operands prepared once for the whole batch.
 template <typename OutT>
 int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, const OperandMaps &ma,
-           const OperandMaps &mb, float beta, OutT *C, int64_t rsC, int64_t csC, bool pair, cudaStream_t s,
+           const OperandMaps &mb, float beta, OutT *C, int64_t rsC, int64_t csC, cudaStream_t s,
            const Epilogue &epi, const F16Scales *f16 = nullptr, bool after_prep = false, const BatchArgs *bat = nullptr,
            bool a_shared = false, bool b_shared = false) {
   TcLaunch l;
   l.a0 = ma.p0; l.a1 = ma.p1; l.b0 = mb.p0; l.b1 = mb.p1;
   l.a_mn = ma.mn_major; l.b_mn = mb.mn_major;
-  l.pair = pair;
   l.pdl = c.pdl && after_prep;   // the preceding kernel of the stream is one of ours and calls launch_dependents
   l.dev = c.dev; l.sm_count = c.sm_count; l.stream = s;
   TcParams &p = l.p;
   p.M = M; p.N = N; p.K = K; p.alpha = alpha; p.beta = beta;
-  p.C = C; p.rsC = rsC; p.csC = csC; p.zero = 0; p.epi = epi;
+  p.C = C; p.rsC = rsC; p.csC = csC; p.epi = epi;
   if (f16) { p.amax_a = f16->a; p.amax_b = f16->b; }
   if (bat) {
     l.batched = true;
@@ -695,8 +689,8 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
   }
   const int npass = (kind == TC_TF32X3 || kind == TC_F16X3) ? 3 : 1;
   const TcPlanCfg cfg{c.kc_faithful, c.raster_g, c.splitk_enabled, c.sm_count};
-  if (kind == TC_BF16 || kind == TC_F16X3) tc_plan<2, std::is_same<OutT, float>::value>(p, npass, pair, cfg);
-  else tc_plan<4, std::is_same<OutT, float>::value>(p, npass, pair, cfg);
+  if (kind == TC_BF16 || kind == TC_F16X3) tc_plan<2, std::is_same<OutT, float>::value>(p, npass, cfg);
+  else tc_plan<4, std::is_same<OutT, float>::value>(p, npass, cfg);
   if (c.dyn_sched) {
     p.sched = static_cast<unsigned int *>(c.sched.ptr) + 2 * c.sched_next;
     c.sched_next = (c.sched_next + 1) % kSchedSlots;
@@ -725,17 +719,16 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
     if constexpr (std::is_same<OutT, float>::value) {
       // units past the direct tiles write raw partial sums to tile-local planes of the workspace (tc_params.h); a second
       // kernel adds the planes of those tiles and applies alpha / beta / epilogue
-      const int64_t ws_floats = tc_split_ws_floats(p, pair);
+      const int64_t ws_floats = tc_split_ws_floats(p);
       if ((rc = ensure(c.splitk, static_cast<size_t>(ws_floats) * sizeof(float)))) return rc;
       p.split_ws = static_cast<float *>(c.splitk.ptr);
       if ((rc = launch(l))) return rc;
       const int n_tail = p.num_m_blocks * p.num_n_blocks * p.batch - p.n_direct;
-      const int tile_m = pair ? 2 * TC_BLOCK_M : TC_BLOCK_M;
-      const int64_t items = (static_cast<int64_t>(n_tail) * tile_m * (TC_BLOCK_N / 4) + 255) / 256;
+      const int64_t items = (static_cast<int64_t>(n_tail) * TC_BLOCK_M * (TC_BLOCK_N / 4) + 255) / 256;
       auto reduce = [&](auto batched) {
         splitk_tail_reduce_kernel<decltype(batched)::value><<<grid_for(c, items, 8), 256, 0, s>>>(
             static_cast<const float *>(c.splitk.ptr), p.k_splits, n_tail, p.n_direct, p.num_m_blocks, p.num_n_blocks, p.raster_g,
-            tile_m, M, N, alpha, beta, C, rsC, csC, p.epi.bias, p.epi.bias_per_row, p.epi.act, p.bsC);
+            M, N, alpha, beta, C, rsC, csC, p.epi.bias, p.epi.bias_per_row, p.epi.act, p.bsC);
       };
       if (bat) reduce(std::true_type());
       else reduce(std::false_type());
@@ -783,15 +776,13 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
       (rc = f16_scales(c, batch_of(oa).n * M, batch_of(ob).n * N, &f16_b_off)))
     return rc;
   if ((rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s, opA))) return rc;
-  // clusters of two CTAs (256 x 128 tiles) when enabled and there are at least two 128-row blocks (never in a batched launch)
-  const bool pair = !bat && c.cta_pair && M > TC_BLOCK_M;
   if (b_ready) CUDA_TRY(cudaStreamWaitEvent(s, b_ready, 0));
   if ((rc = prepare_operand<SRC_ESZ>(c, ob, mode, ws_of_B(c, f16_b_off), TC_BLOCK_N, &mb, &used_ws, s, opB))) return rc;
   const int prep_launches = prep.launches();
   if ((rc = prep.close())) return rc;
   const F16Scales f16{static_cast<const uint32_t *>(c.f16s.ptr), static_cast<const uint32_t *>(c.f16s.ptr) + f16_b_off};
   // (with profiling on, an event record sits between the last preparation kernel and the GEMM: no dependent launch then)
-  rc = tc_run<OutT>(c, kind, M, N, K, alpha, ma, mb, beta, C, rsC, csC, pair, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
+  rc = tc_run<OutT>(c, kind, M, N, K, alpha, ma, mb, beta, C, rsC, csC, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
                     prep_launches > 0 && !c.profiling, bat, a_shared, b_shared);
   if (rc) return rc;
   if (used_ws) CUDA_TRY(cudaEventRecord(c.ws_free, s));
@@ -881,7 +872,6 @@ int gemm_packed_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c.stream;
   {
     std::lock_guard<std::mutex> lk(c.mu);
-    const bool pair = c.cta_pair && M > TC_BLOCK_M;
     OperandMaps ma, mb;
     F16Scales f16;
     bool used_ws = false;
@@ -901,7 +891,7 @@ int gemm_packed_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A
       f16.a = static_cast<const uint32_t *>(c.f16s.ptr);
     }
     if ((rc = packed_maps(c, packedB, N, K, TC_BLOCK_N, &mb, &f16.b))) return rc;
-    if ((rc = tc_run<float>(c, TC_F16X3, M, N, K, alpha, ma, mb, beta, C, rsC, csC, pair, s, Epilogue(), &f16,
+    if ((rc = tc_run<float>(c, TC_F16X3, M, N, K, alpha, ma, mb, beta, C, rsC, csC, s, Epilogue(), &f16,
                             prep_launches > 0 && !c.profiling)))
       return rc;
     if (used_ws) CUDA_TRY(cudaEventRecord(c.ws_free, s));
@@ -1289,7 +1279,6 @@ int host_gemm_f32_pipelined(Ctx &c, int64_t M, int64_t N, int64_t K, float alpha
   // f16x3: B's abs-max words are written once, A's (one per row of the panel) are rewritten by every panel's preparation --
   // after the previous panel's GEMM, whose epilogue reads them, because everything of a panel runs on the compute stream
   const SplitMode mode = split_mode(kind);
-  const bool pair = c.cta_pair && panel_rows > TC_BLOCK_M && M > TC_BLOCK_M;
   // staging buffers / workspace may still be in use by an earlier call
   CUDA_TRY(cudaStreamWaitEvent(up, c.ws_free, 0));
   CUDA_TRY(cudaStreamWaitEvent(cmp, c.ws_free, 0));
@@ -1323,9 +1312,7 @@ int host_gemm_f32_pipelined(Ctx &c, int64_t M, int64_t N, int64_t K, float alpha
     OperandMaps ma;
     Operand oa{dA + m0 * rsA, mp, K, rsA, csA};
     if ((rc = prepare_operand<4>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, cmp))) return rc;
-    // B's tensor maps were built for `pair` (128- vs 256-column boxes): every panel, however
-    // short, must run the same kernel variant
-    rc = tc_run<float>(c, kind, mp, N, K, alpha, ma, mb, beta, dC + m0 * rsC, rsC, csC, pair, cmp, Epilogue(),
+    rc = tc_run<float>(c, kind, mp, N, K, alpha, ma, mb, beta, dC + m0 * rsC, rsC, csC, cmp, Epilogue(),
                        f16x3 ? &f16 : nullptr, mode != SPLIT_NONE && !c.profiling);
     if (rc) return rc;
     CUDA_TRY(cudaEventRecord(c.panel_ev[panels + pnl], cmp));

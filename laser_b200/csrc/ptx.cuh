@@ -1,5 +1,5 @@
-// ptx.cuh -- thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), clusters,
-// wgmma (fence / mma_async / commit / wait) and the wgmma shared-memory matrix descriptor.
+// ptx.cuh -- thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), programmatic dependent
+// launch, wgmma (fence / mma_async / commit / wait) and the wgmma shared-memory matrix descriptor.
 // Hand-written; bit layouts follow the PTX ISA "asynchronous warpgroup level matrix" chapter.
 #pragma once
 
@@ -8,7 +8,7 @@
 #include <stdint.h>
 
 #ifdef LB200_HOST_EMULATION
-// tests/emu: the same names backed by a functional model of mbarrier / TMA / wgmma / clusters on
+// tests/emu: the same names backed by a functional model of mbarrier / TMA / wgmma on
 // host threads (test infrastructure; see tests/emu/ptx_emu.h)
 #include "ptx_emu.h"
 #else
@@ -204,59 +204,7 @@ __device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t a_
       : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
 
-// ------------------------------------------------------------ clusters of two CTAs
-// In a cluster launch the shared-window address of a CTA's own shared memory carries the
-// CTA's rank in bit 24; clearing it names the same offset in the even (leader) CTA of a pair.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive (count 1) on the LEADER CTA's copy of this mbarrier, from either CTA of the pair
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t *bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-// shared::cluster address of the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t cluster_addr(const void *p, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
-  return r;
-}
-// arrive (count 1, release at cluster scope) on the copy of this mbarrier in CTA `rank`: orders this thread's earlier
-// writes -- including st.shared::cluster into that CTA -- before the arrival
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t rank) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr(bar, rank)) : "memory");
-}
-// arrive WITHOUT release semantics (no memory barrier is emitted): for consumers that only signal "I have read the slot";
-// `count` is threaded through a register so that the caller can make the arrival data-dependent on what it read
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint64_t *bar, uint32_t rank, uint32_t count) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0], %1;" ::"r"(cluster_addr(bar, rank)), "r"(count)
-               : "memory");
-}
-// wait on this CTA's mbarrier with acquire at cluster scope (the data it guards was written by the peer CTA)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t *bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, P;\n\t"
-        "}\n"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-// 32-bit store into the shared memory of CTA `rank` (same offset as `p` in this CTA)
-__device__ __forceinline__ void st_shared_cluster_s32(int *p, uint32_t rank, int v) {
-  asm volatile("st.shared::cluster.s32 [%0], %1;" ::"r"(cluster_addr(p, rank)), "r"(v) : "memory");
-}
+// ------------------------------------------------------------ programmatic dependent launch
 // programmatic dependent launch: wait until the kernels this launch depends on have completed and flushed (no-op when
 // the kernel was launched without the attribute); launch_dependents lets the next kernel of the stream start its prologue
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

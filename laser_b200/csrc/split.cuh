@@ -532,16 +532,16 @@ pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr
 }
 
 // Second half of a split-K GEMM (tc_params.h): C <- act(alpha * sum_s ws[s][i] + beta * C + bias) over the split tiles
-// n_direct + i, i < n_tail, planes added in the fixed order s = 0 .. S-1 (deterministic).  ws: [S][n_tail][tile_m][TC_BLOCK_N]
+// n_direct + i, i < n_tail, planes added in the fixed order s = 0 .. S-1 (deterministic).  ws: [S][n_tail][TC_BLOCK_M][TC_BLOCK_N]
 // fp32, tile-local.  Item = four consecutive columns of one tile row.  BATCHED: tile t of the launch is tile t % (num_m * num_n)
 // of problem t / (num_m * num_n), whose C starts bsC elements after the previous problem's (tc_params.h).
 template <bool BATCHED = false>
 __global__ void __launch_bounds__(256)
 splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n_direct, int num_m, int num_n, int raster_g,
-                          int tile_m, int64_t M, int64_t N, float alpha, float beta, float *__restrict__ C, int64_t rsC,
+                          int64_t M, int64_t N, float alpha, float beta, float *__restrict__ C, int64_t rsC,
                           int64_t csC, const float *__restrict__ bias, int bias_per_row, int act, int64_t bsC = 0) {
   constexpr int V = TC_BLOCK_N / 4;   // float4 per tile row
-  const int64_t per_tile = static_cast<int64_t>(tile_m) * V;
+  const int64_t per_tile = static_cast<int64_t>(TC_BLOCK_M) * V;
   const int64_t total = static_cast<int64_t>(n_tail) * per_tile;
   const int64_t plane = total * 4;    // floats between consecutive split planes
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
@@ -557,7 +557,7 @@ splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n
       Cb += b * bsC;
     }
     tile_coords(t, num_m, num_n, raster_g, mb, nb);
-    const int64_t r = static_cast<int64_t>(mb) * tile_m + r_l, c = static_cast<int64_t>(nb) * TC_BLOCK_N + 4 * c4;
+    const int64_t r = static_cast<int64_t>(mb) * TC_BLOCK_M + r_l, c = static_cast<int64_t>(nb) * TC_BLOCK_N + 4 * c4;
     if (r >= M || c >= N) continue;
     const float *src = ws + i * 4;
     float4 sum = *reinterpret_cast<const float4 *>(src);

@@ -1,5 +1,5 @@
-// tc_f16x3.cu -- the eight instantiations (operand major-ness x single CTA / cluster of two) of
-// gemm_tc_kernel<2, ptx::kFmtF16, 3, float, true>, and the four of gemm_tc_batched_kernel (operand major-ness)
+// tc_f16x3.cu -- the four instantiations (operand major-ness) of gemm_tc_kernel<2, ptx::kFmtF16, 3, ..., float, true>, and
+// the four batched ones
 #include "tc_launch_impl.cuh"
 
 namespace lb200 {

@@ -13,8 +13,7 @@ struct TcLaunch {
   CUtensorMap a0, a1, b0, b1;   // piece 0 (hi / the operand itself) and piece 1 (lo) of A and B
   TcParams p;
   bool a_mn = false, b_mn = false;   // operand major-ness
-  bool pair = false;                 // clusters of two CTAs sharing one tile scheduler
-  bool batched = false;              // p.batch problems, rank-3 tensor maps (fp32 families, single CTAs: tc_params.h)
+  bool batched = false;              // p.batch problems, rank-3 tensor maps (fp32 families: tc_params.h)
   bool pdl = false;                  // programmatic dependent launch: overlap the prologue with the preceding kernel's tail
   int dev = 0, sm_count = 0;
   cudaStream_t stream = nullptr;

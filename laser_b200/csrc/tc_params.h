@@ -16,7 +16,7 @@ constexpr int TC_BLOCK_M = 128;
 constexpr int TC_BLOCK_N = 128;
 constexpr int TC_ROW_BYTES = 128;  // one swizzle row; BLOCK_K = 128 / sizeof(element)
 constexpr int TC_A_TILE_BYTES = TC_BLOCK_M * TC_ROW_BYTES;  // 16 KB: 128 rows x 128 B
-template <int NPASS, bool PAIR> struct TcCfg {
+template <int NPASS> struct TcCfg {
   static constexpr int PIECES = (NPASS == 3) ? 2 : 1;
   static constexpr int B_TILE_BYTES = TC_BLOCK_N * TC_ROW_BYTES;
   static constexpr int A_STAGE_BYTES = PIECES * TC_A_TILE_BYTES;
@@ -49,7 +49,6 @@ struct TcParams {
   void *C;
   int64_t rsC, csC;
   int kb_per_block;   // k-tiles per accumulation block of the wgmma registers (>= 1)
-  uint32_t zero;      // always 0; opaque to the compiler (see the epilogue)
   int raster_g;       // m-blocks per raster group (see tile_coords)
   Epilogue epi;
   // split-K.  Tiles [0, n_direct) (raster order, tile_coords) are computed over all of K and stored through the epilogue
@@ -62,12 +61,12 @@ struct TcParams {
   int n_direct;          // == num_m_blocks * num_n_blocks when nothing is split
   int k_splits;          // >= 1
   int kb_per_split;      // k-tiles per split
-  float *split_ws = nullptr;   // [k_splits][split tiles][tile rows][TC_BLOCK_N] fp32
-  int num_m_blocks, num_n_blocks;  // output tiles: 128 x 128, or 256 x 128 per cluster of two CTAs
+  float *split_ws = nullptr;   // [k_splits][split tiles][TC_BLOCK_M][TC_BLOCK_N] fp32
+  int num_m_blocks, num_n_blocks;  // output tiles of 128 x 128
   // SCALED: fp32 bits of the largest finite |a| of row i of A / |b| of column j of B (f16_scale.cuh)
   const uint32_t *amax_a = nullptr, *amax_b = nullptr;
-  // tile scheduler: word 0 = next unit (atomicAdd), word 1 = pairs that have drawn their last unit (the last one zeroes
-  // both words for the next launch that uses this slot).  nullptr: static round-robin (unit = pair index + i * pairs)
+  // tile scheduler: word 0 = next unit (atomicAdd), word 1 = CTAs that have drawn their last unit (the last one zeroes
+  // both words for the next launch that uses this slot).  nullptr: static round-robin (unit = CTA index + i * CTAs)
   unsigned int *sched = nullptr;
   // batched launch (gemm_tc_kernel<..., BATCHED = true>): `batch` problems of M x N x K.  Tile t of the launch is tile
   // t % (num_m_blocks * num_n_blocks) of problem t / (num_m_blocks * num_n_blocks); split-K and the raster order apply to
@@ -80,8 +79,8 @@ struct TcParams {
 };
 
 // raster order of the output tiles: groups of G m-blocks sweep n together, so that the concurrently resident tiles (132 of
-// 128 x 128 on an H100 SXM, or 66 cluster tiles of 256 x 128) cover a compact patch, which limits the A + B panels one wave
-// pulls through L2 (G = 16 single-CTA tiles / 8 cluster tiles = 2048 rows)
+// 128 x 128 on an H100 SXM) cover a compact patch, which limits the A + B panels one wave pulls through L2 (G = 16 tiles =
+// 2048 rows)
 LB200_HD inline void tile_coords(int t, int num_m, int num_n, int G, int &mb, int &nb) {
   const int per_group = G * num_n;
   const int g = t / per_group;
@@ -102,7 +101,7 @@ struct TcPlanCfg {
   int tail_min_k = 2048;   // shortest K for which the remainder behind full waves is split
 };
 template <int ESZ, bool OUT_F32>
-inline void tc_plan(TcParams &p, int npass, bool pair, const TcPlanCfg &cfg) {
+inline void tc_plan(TcParams &p, int npass, const TcPlanCfg &cfg) {
   const int block_k = TC_ROW_BYTES / ESZ;  // k-tile
   const int num_kb = static_cast<int>((p.K + block_k - 1) / block_k);
   {
@@ -114,9 +113,8 @@ inline void tc_plan(TcParams &p, int npass, bool pair, const TcPlanCfg &cfg) {
     if (p.kb_per_block < 1) p.kb_per_block = 1;
     if (p.kb_per_block > num_kb) p.kb_per_block = num_kb;
   }
-  p.raster_g = cfg.raster_g > 0 ? cfg.raster_g : (pair ? 8 : 16);
-  const int tile_m = pair ? 2 * TC_BLOCK_M : TC_BLOCK_M;
-  p.num_m_blocks = static_cast<int>((p.M + tile_m - 1) / tile_m);
+  p.raster_g = cfg.raster_g > 0 ? cfg.raster_g : 16;
+  p.num_m_blocks = static_cast<int>((p.M + TC_BLOCK_M - 1) / TC_BLOCK_M);
   p.num_n_blocks = static_cast<int>((p.N + TC_BLOCK_N - 1) / TC_BLOCK_N);
   // ---- split-K (fp32 output only): too few output tiles to fill the machine and a long K, or a thin last wave ----
   const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks * p.batch;
@@ -124,7 +122,7 @@ inline void tc_plan(TcParams &p, int npass, bool pair, const TcPlanCfg &cfg) {
   p.kb_per_split = num_kb;
   p.n_direct = static_cast<int>(tiles);
   p.split_ws = nullptr;
-  const int units = pair ? cfg.sm_count / 2 : cfg.sm_count;
+  const int units = cfg.sm_count;
   if constexpr (OUT_F32) {
     const int blocks = (num_kb + p.kb_per_block - 1) / p.kb_per_block;   // accumulation blocks along K
     // every split keeps >= 512 K-elements
@@ -152,10 +150,9 @@ inline int64_t tc_units(const TcParams &p) {
   const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks * p.batch;
   return p.n_direct + (tiles - p.n_direct) * p.k_splits;
 }
-inline int64_t tc_split_ws_floats(const TcParams &p, bool pair) {
+inline int64_t tc_split_ws_floats(const TcParams &p) {
   const int64_t tiles = static_cast<int64_t>(p.num_m_blocks) * p.num_n_blocks * p.batch;
-  const int64_t tile_m = pair ? 2 * TC_BLOCK_M : TC_BLOCK_M;
-  return (tiles - p.n_direct) * p.k_splits * tile_m * TC_BLOCK_N;
+  return (tiles - p.n_direct) * p.k_splits * TC_BLOCK_M * TC_BLOCK_N;
 }
 
 }  // namespace lb200

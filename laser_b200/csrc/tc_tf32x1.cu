@@ -1,5 +1,5 @@
-// tc_tf32x1.cu -- the two instantiations (K-major operands x single CTA / cluster of two) of gemm_tc_kernel<4, ptx::kFmtBF16, 1, float, false>,
-// and gemm_tc_batched_kernel
+// tc_tf32x1.cu -- the instantiation (K-major operands) of gemm_tc_kernel<4, ptx::kFmtBF16, 1, ..., float, false>, and the
+// batched one
 #include "tc_launch_impl.cuh"
 
 namespace lb200 {

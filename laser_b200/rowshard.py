@@ -20,8 +20,8 @@ __all__ = ["partition_rows", "Comm", "comm_init_all", "comm_init_rank", "comm_fr
 
 
 def partition_rows(M, world_size, align=256):
-    """[(start, stop)] per rank: ceil(M / world) rounded up to the CTA-pair tile height; the last ranks take what is
-    left (possibly nothing).  Same rule as laser_b200_rowshard_partition (align = 256)."""
+    """[(start, stop)] per rank: ceil(M / world) rounded up to a multiple of 256 rows (the partition the library has always
+    used); the last ranks take what is left (possibly nothing).  Same rule as laser_b200_rowshard_partition (align = 256)."""
     per = -(-M // world_size)
     per = -(-per // align) * align
     out = []

@@ -26,16 +26,13 @@ template <typename... KArgs, typename... Args>
 inline void launch_kernel(void (*kernel)(KArgs...), unsigned grid, unsigned block, cudaStream_t s, Args &&...args) {
   emu_launch_kernel(kernel, grid, block, 0, s, static_cast<Args &&>(args)...);
 }
-// cudaLaunchKernelEx with a cluster dimension (the wgmma kernel)
+// cudaLaunchKernelEx (the wgmma kernel; its launch attributes have no functional effect here)
 template <typename... KArgs, typename... Args>
 inline cudaError_t emu_launch_ex(const cudaLaunchConfig_t *cfg, void (*kernel)(KArgs...), Args &&...args) {
-  unsigned cluster = 1;
-  for (unsigned i = 0; i < cfg->numAttrs; ++i)
-    if (cfg->attrs[i].id == cudaLaunchAttributeClusterDimension) cluster = cfg->attrs[i].val.clusterDim.x;
   if (cfg->dynamicSmemBytes > emu::kDynSmemBytes) return cudaErrorInvalidValue;
   std::lock_guard<std::recursive_mutex> device_lk(emu::launch_mu);   // reset + launch are one step of the one emulated device
   emu::reset_state();
-  emu::launch(cfg->gridDim.x, cfg->blockDim.x, [=]() { kernel(static_cast<KArgs>(args)...); }, cluster);
+  emu::launch(cfg->gridDim.x, cfg->blockDim.x, [=]() { kernel(static_cast<KArgs>(args)...); });
   return cudaSuccess;
 }
 

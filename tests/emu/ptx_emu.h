@@ -1,11 +1,11 @@
 // ptx_emu.h -- TEST INFRASTRUCTURE: a functional model of the PTX that laser_b200/csrc/ptx.cuh
-// wraps (mbarrier, cp.async.bulk.tensor, wgmma, clusters of two CTAs), under the same names, so
+// wraps (mbarrier, cp.async.bulk.tensor, wgmma), under the same names, so
 // that gemm_tc.cuh -- the wgmma kernel -- can be compiled by g++ and run on host threads
 // (cuda_emu.h).  What the model checks: the producer / consumer protocol (barrier counts, phases,
 // stage rings: a protocol error shows up as a deadlock or as a wrong sum), the tile scheduler,
 // raster and split-K ranges, the k-block bookkeeping of every mode, operand addressing through the
 // descriptors' start / LBO / SBO fields, the accumulator fragment layout the epilogue assumes,
-// out-of-bounds zero fill, the cluster's ownership of rows, and every epilogue path.  What it
+// out-of-bounds zero fill, and every epilogue path.  What it
 // cannot check: anything that is a property of the silicon -- the 128-byte swizzle patterns (tiles
 // are kept unswizzled here, on both the TMA and the MMA side), instruction encodings, the
 // asynchrony of wgmma (an instruction completes when it is issued here), memory-proxy fences,
@@ -24,8 +24,8 @@
 #include <map>
 #include <mutex>
 
-// dynamic shared memory of the kernel: this CTA's buffer
-#define LB200_DYN_SMEM(T, name) T *name = reinterpret_cast<T *>(emu::dyn_smem_ptr())
+// dynamic shared memory of the kernel
+#define LB200_DYN_SMEM(T, name) T *name = reinterpret_cast<T *>(emu::dyn_smem)
 
 namespace emu {
 
@@ -80,27 +80,15 @@ inline void mb_complete_tx(const void *bar, long bytes) {
   b.tx -= bytes;
   mb_check(b);
 }
-// the same offset in the shared memory of CTA `rank` of the cluster
-template <typename T>
-inline T *peer_ptr(T *p, unsigned rank) {
-  const unsigned char *q = reinterpret_cast<const unsigned char *>(p);
-  for (unsigned r = 0; r < kMaxCluster; ++r)
-    if (q >= dyn_smem[r] && q < dyn_smem[r] + kDynSmemBytes)
-      return reinterpret_cast<T *>(dyn_smem[rank] + (q - dyn_smem[r]));
-  std::fprintf(stderr, "emu: pointer %p is not in shared memory\n", static_cast<const void *>(p));
-  std::abort();
-}
 }  // namespace emu
 
 namespace lb200 {
 namespace ptx {
 
-// shared-window address: offset inside the CTA's shared memory, CTA rank in bit 24
+// shared-window address: offset inside the CTA's shared memory
 inline uint32_t smem_u32(const void *p) {
   const unsigned char *q = static_cast<const unsigned char *>(p);
-  for (unsigned r = 0; r < emu::kMaxCluster; ++r)
-    if (q >= emu::dyn_smem[r] && q < emu::dyn_smem[r] + emu::kDynSmemBytes)
-      return static_cast<uint32_t>(q - emu::dyn_smem[r]) | (r << 24);
+  if (q >= emu::dyn_smem && q < emu::dyn_smem + emu::kDynSmemBytes) return static_cast<uint32_t>(q - emu::dyn_smem);
   std::fprintf(stderr, "emu: smem_u32 of a pointer outside shared memory\n");
   std::abort();
 }
@@ -140,8 +128,8 @@ inline void mbar_wait(uint64_t *bar, uint32_t parity) {   // blocking (hundreds 
   emu::MBarrier &b = emu::mb_get(bar);
   // a protocol error is a deadlock: past the limit, report the barrier and the waiting thread instead of hanging
   if (!emu::mb_cv.wait_for(lk, std::chrono::seconds(mbar_wait_limit_s()), [&]() { return b.phase != parity; })) {
-    std::fprintf(stderr, "emu: deadlock: thread %u of CTA rank %u waits for parity %u of the mbarrier at shared offset %u "
-                 "(pending %d of %d arrivals, tx %ld)\n", emu::t_idx.x, emu::cta_rank, parity,
+    std::fprintf(stderr, "emu: deadlock: thread %u of CTA %u waits for parity %u of the mbarrier at shared offset %u "
+                 "(pending %d of %d arrivals, tx %ld)\n", emu::t_idx.x, emu::b_idx.x, parity,
                  static_cast<unsigned>(smem_u32(bar) & 0xFFFFFF), b.pending, b.init_count, b.tx);
     emu::mb_cv.wait_for(lk, std::chrono::seconds(5));   // the other blocked threads report too
     std::abort();
@@ -159,7 +147,7 @@ inline void tma_copy_box(void *smem_dst, const CUtensorMap *map, int32_t c0, int
   if (m.magic != emu::kMapMagic) { std::fprintf(stderr, "emu: not an emulated tensor map\n"); std::abort(); }
   unsigned char *dst = static_cast<unsigned char *>(smem_dst);
   {   // the destination must be this CTA's shared memory, whole box inside it, swizzle-atom (1024 B) aligned
-    const unsigned char *lo = emu::dyn_smem[emu::cta_rank];
+    const unsigned char *lo = emu::dyn_smem;
     const size_t box_bytes = static_cast<size_t>(m.box0) * m.box1 * m.esz;
     if (dst < lo || dst + box_bytes > lo + emu::kDynSmemBytes || ((dst - lo) & 1023)) {
       std::fprintf(stderr, "emu: TMA destination outside this CTA's shared memory or not 1024-byte aligned\n");
@@ -216,7 +204,7 @@ inline void wgmma_fence() {}
 inline void wgmma_commit() {}
 // .sync.aligned: every lane of the warp has issued (and, in this model, completed) its MMAs before any lane goes on -- lane 0
 // then releases the stage for the whole warp
-template <int N> inline void wgmma_wait() { pthread_barrier_wait(&emu::warp_barrier[emu::cta_rank][emu::t_idx.x >> 5]); }
+template <int N> inline void wgmma_wait() { pthread_barrier_wait(&emu::warp_barrier[emu::t_idx.x >> 5]); }
 inline void wgmma_hold(float (&)[64]) {}
 
 constexpr uint32_t kLayoutSw128 = 1;
@@ -274,7 +262,7 @@ inline float operand_elem(const unsigned char *cta_smem, uint64_t desc, bool mn_
 inline void wgmma_model(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d, int E, uint32_t fmt, bool a_mn, bool b_mn) {
   if (E == 4 && (a_mn || b_mn)) { std::fprintf(stderr, "emu: tf32 operands must be K-major\n"); std::abort(); }
   const unsigned t = emu::t_idx.x & 127u, w = t >> 5, lane = t & 31u;
-  const unsigned char *sm = emu::dyn_smem[emu::cta_rank];
+  const unsigned char *sm = emu::dyn_smem;
   const int KI = 32 / E;
   float a[2][16], b[32][16];
   for (int h = 0; h < 2; ++h)
@@ -297,17 +285,7 @@ template <int TA, int TB>
 inline void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t scale_d) { wgmma_model(d, ad, bd, scale_d, 2, kFmtBF16, TA, TB); }
 inline void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t scale_d) { wgmma_model(d, ad, bd, scale_d, 4, kFmtTF32, false, false); }
 
-// ------------------------------------------------------------ clusters of two CTAs
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-inline uint32_t cluster_ctarank() { return emu::cta_rank; }
-inline void cluster_sync() { pthread_barrier_wait(&emu::cluster_barrier); }
-inline void mbar_arrive_leader(uint64_t *bar) { emu::mb_arrive(emu::peer_ptr(bar, 0), 0); }
-inline void mbar_arrive_cluster(uint64_t *bar, uint32_t rank) { emu::mb_arrive(emu::peer_ptr(bar, rank), 0); }
-inline void mbar_arrive_cluster_relaxed(uint64_t *bar, uint32_t rank, uint32_t count) {
-  for (uint32_t i = 0; i < count; ++i) emu::mb_arrive(emu::peer_ptr(bar, rank), 0);
-}
-inline void mbar_wait_cluster(uint64_t *bar, uint32_t parity) { mbar_wait(bar, parity); }
-inline void st_shared_cluster_s32(int *p, uint32_t rank, int v) { *reinterpret_cast<volatile int *>(emu::peer_ptr(p, rank)) = v; }
+// ------------------------------------------------------------ programmatic dependent launch
 inline void griddep_wait() {}
 inline void griddep_launch_dependents() {}
 
@@ -315,16 +293,16 @@ inline void griddep_launch_dependents() {}
 // mma.sync.aligned.m8n8k4.row.col.f64 (gemm_dmma.cuh): lane l holds A[l / 4][l % 4], B[l % 4][l / 4] and the two accumulators
 // D[l / 4][2 * (l % 4) + {0, 1}]; per output element the four steps of the FMA chain in k order
 inline void dmma_m8n8k4(double &d0, double &d1, double a, double b) {
-  const unsigned t = emu::t_idx.x, w = t >> 5, r = emu::cta_rank, base = t & ~31u, lane = t & 31u;
-  emu::warp_scratch_d[r][0][t] = a;
-  emu::warp_scratch_d[r][1][t] = b;
-  pthread_barrier_wait(&emu::warp_barrier[r][w]);
+  const unsigned t = emu::t_idx.x, w = t >> 5, base = t & ~31u, lane = t & 31u;
+  emu::warp_scratch_d[0][t] = a;
+  emu::warp_scratch_d[1][t] = b;
+  pthread_barrier_wait(&emu::warp_barrier[w]);
   const unsigned row = lane >> 2, c0 = 2 * (lane & 3);
   for (unsigned k = 0; k < 4; ++k) {
-    const double ak = emu::warp_scratch_d[r][0][base + row * 4 + k];
-    d0 = std::fma(ak, emu::warp_scratch_d[r][1][base + c0 * 4 + k], d0);
-    d1 = std::fma(ak, emu::warp_scratch_d[r][1][base + (c0 + 1) * 4 + k], d1);
+    const double ak = emu::warp_scratch_d[0][base + row * 4 + k];
+    d0 = std::fma(ak, emu::warp_scratch_d[1][base + c0 * 4 + k], d0);
+    d1 = std::fma(ak, emu::warp_scratch_d[1][base + (c0 + 1) * 4 + k], d1);
   }
-  pthread_barrier_wait(&emu::warp_barrier[r][w]);
+  pthread_barrier_wait(&emu::warp_barrier[w]);
 }
 }  // namespace lb200

@@ -48,11 +48,11 @@ void emu_pack_general_u16(const uint16_t *src, int64_t R, int64_t Cc, int64_t sr
                           int read_along_r, int grid) {
   emu::launch(grid, 256, [=]() { pack_general_kernel<uint16_t, 0>(src, R, Cc, sr, sc, dst, nullptr, ld, read_along_r); });
 }
-void emu_splitk_tail_reduce(const float *ws, int S, int n_tail, int n_direct, int num_m, int num_n, int raster_g, int tile_m,
+void emu_splitk_tail_reduce(const float *ws, int S, int n_tail, int n_direct, int num_m, int num_n, int raster_g,
                             int64_t M, int64_t N, float alpha, float beta, float *C, int64_t rsC, int64_t csC, const float *bias,
                             int bias_per_row, int act, int grid) {
   emu::launch(grid, 256, [=]() {
-    splitk_tail_reduce_kernel(ws, S, n_tail, n_direct, num_m, num_n, raster_g, tile_m, M, N, alpha, beta, C, rsC, csC, bias,
+    splitk_tail_reduce_kernel(ws, S, n_tail, n_direct, num_m, num_n, raster_g, M, N, alpha, beta, C, rsC, csC, bias,
                               bias_per_row, act);
   });
 }

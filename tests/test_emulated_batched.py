@@ -133,11 +133,12 @@ def test_general_gather(emu, op, mode):
 
 
 def test_batched_gemm_kernels_issue_3d_tma_loads():
-    """every instantiation of the batched tensor-core kernel loads through 3-D tensor maps only, every instantiation of the
-    one-problem kernel through 2-D maps only"""
+    """every batched instantiation of the tensor-core kernel (template argument BATCHED = true) loads through 3-D tensor
+    maps only, every one-problem instantiation through 2-D maps only"""
     exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(exe):
-        pytest.skip("cuobjdump not installed")
+    filt = shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
+    if not os.path.exists(exe) or not os.path.exists(filt):
+        pytest.skip("cuobjdump / cu++filt not installed")
     out = subprocess.run([exe, "-sass", _L.lib_path()], capture_output=True, text=True, check=True).stdout
     loads, cur = {}, None
     for line in out.splitlines():
@@ -148,15 +149,20 @@ def test_batched_gemm_kernels_issue_3d_tma_loads():
         elif cur:
             for d in re.findall(r"UTMALDG\.(\dD)", line):
                 loads[cur][d] += 1
+    syms = [s for s in loads if "gemm_tc_kernel" in s]
+    names = subprocess.run([filt], input="\n".join(syms), capture_output=True, text=True, check=True).stdout.splitlines()
     batched = plain = 0
-    for sym, cnt in loads.items():
-        if "gemm_tc_batched_kernel" in sym:
+    for sym, name in zip(syms, names):
+        # gemm_tc_kernel<ESZ, FMT16, NPASS, A_MN, B_MN, OutT, SCALED, BATCHED>(...)
+        m = re.match(r"void lb200::gemm_tc_kernel<.*, \(bool\)([01])>\(", name)
+        assert m, name
+        if m.group(1) == "1":
             batched += 1
-            assert set(cnt) == {"3D"}, (sym, cnt)
-        elif "gemm_tc_kernel" in sym:
+            assert set(loads[sym]) == {"3D"}, (name, loads[sym])
+        else:
             plain += 1
-            assert set(cnt) == {"2D"}, (sym, cnt)
-    assert batched == 6 and plain == 20, (batched, plain)   # batched: f16x3 x 4 majors, tf32x3, tf32x1
+            assert set(loads[sym]) == {"2D"}, (name, loads[sym])
+    assert batched == 6 and plain == 10, (batched, plain)   # batched: f16x3 x 4 majors, tf32x3, tf32x1
 
 
 def test_batched_file_against_the_host_emulated_library():

@@ -44,7 +44,6 @@ def test_split_k_planning_and_reduce(emulated_lib):
 
 @pytest.mark.parametrize("env", [dict(LASER_B200_PANEL_ROWS=512), dict(LASER_B200_PANEL_TAPER=1),
                                  dict(LASER_B200_PANEL_ROWS=512, LASER_B200_PANEL_TAPER=1),
-                                 dict(LASER_B200_CTA_PAIR=0), dict(LASER_B200_CTA_PAIR=1),
                                  dict(LASER_B200_F32_MODE="tf32x3"), dict(LASER_B200_DYNSCHED=0),
                                  dict(LASER_B200_KC=64, LASER_B200_RASTER=2)],
                          ids=lambda e: ",".join("%s=%s" % (k.replace("LASER_B200_", ""), v) for k, v in e.items()))
@@ -65,11 +64,11 @@ def test_rowsharded_entry_points_with_a_stand_in_nccl(emulated_lib, ndev, panels
 
 def test_f16x3_mode(emulated_lib):
     """the default fp32 mode: power-of-two scaling from a device-side abs-max, two fp16 pieces, the kernel undoing the
-    scales in its epilogue; range cases included.  Here on a 32-SM machine with clusters of two CTAs (not the default), so
-    that the cluster kernel and split-K take part (the default single-CTA kernel runs the same assertions in
-    test_emulated_python_mirror.py); in
-    the pipelined host-pointer entry every row panel of A gets its own scale"""
-    run(emulated_lib, "f16x3", LASER_B200_EMU_SMS=32, LASER_B200_CTA_PAIR=1, LASER_B200_KC=64)
+    scales in its epilogue; range cases included.  Here on a 32-SM machine with kc = 64 (the default configuration runs the
+    same assertions in test_emulated_python_mirror.py).  None of these products is split along K, on any number of SMs:
+    every split keeps at least 512 K-elements and their K is at most 333; split-K in this mode is
+    test_split_k_planning_and_reduce.  In the pipelined host-pointer entry every row panel of A gets its own scale"""
+    run(emulated_lib, "f16x3", LASER_B200_EMU_SMS=32, LASER_B200_KC=64)
     run(emulated_lib, "host_entry", LASER_B200_F32_MODE="f16x3")
 
 

@@ -25,7 +25,7 @@ def emu():
     L.emu_split_rows_f16x2.argtypes = [ci, vp, i64, i64, i64, vp, vp, i64, vp, ci]
     L.emu_pack_general_f32.argtypes = [ci, vp, i64, i64, i64, i64, vp, vp, i64, ci, ci]
     L.emu_pack_general_u16.argtypes = [vp, i64, i64, i64, i64, vp, i64, ci, ci]
-    L.emu_splitk_tail_reduce.argtypes = [vp, ci, ci, ci, ci, ci, ci, ci, i64, i64, f32, f32, vp, i64, i64, vp, ci, ci, ci]
+    L.emu_splitk_tail_reduce.argtypes = [vp, ci, ci, ci, ci, ci, ci, i64, i64, f32, f32, vp, i64, i64, vp, ci, ci, ci]
     L.emu_fill_uniform_f32.argtypes = [vp, i64, ctypes.c_uint64, f32, f32, ci]
     for n in ("emu_split_rows_tf32", "emu_f16x2_rows_fused", "emu_absmax_mn", "emu_split_rows_f16x2", "emu_pack_general_f32", "emu_pack_general_u16",
               "emu_splitk_tail_reduce", "emu_fill_uniform_f32"):
@@ -155,11 +155,11 @@ def test_pack_general_bf16(emu):
 
 @pytest.mark.parametrize("S,alpha,beta,per_row,act", [(1, 1.0, 0.0, 0, 0), (4, 0.5, -1.25, 0, 0), (3, 1.0, 0.0, 1, 1),
                                                       (5, 2.0, 1.0, 0, 2)])
-@pytest.mark.parametrize("n_direct,tile_m", [(0, 128), (3, 256)])
-def test_splitk_tail_reduce_is_a_fixed_order_sum(emu, S, alpha, beta, per_row, act, n_direct, tile_m):
-    """tile-local planes [S][n_tail][tile_m][BN] (BN = TC_BLOCK_N) of the tiles n_direct.. (raster order, tc_params.h: tile_coords) -> C;
-    the direct tiles of C are not touched"""
-    BN = 128                                             # tc_params.h: TC_BLOCK_N
+@pytest.mark.parametrize("n_direct", [0, 3])
+def test_splitk_tail_reduce_is_a_fixed_order_sum(emu, S, alpha, beta, per_row, act, n_direct):
+    """tile-local planes [S][n_tail][tile_m][BN] (tile_m = TC_BLOCK_M, BN = TC_BLOCK_N) of the tiles n_direct.. (raster order,
+    tc_params.h: tile_coords) -> C; the direct tiles of C are not touched"""
+    tile_m, BN = 128, 128                                # tc_params.h: TC_BLOCK_M, TC_BLOCK_N
     M, N, G = 2 * tile_m + 23, BN + 37, 2               # 3 x 2 tiles, ragged in both directions
     num_m, num_n = -(-M // tile_m), -(-N // BN)
     n_tail = num_m * num_n - n_direct
@@ -168,7 +168,7 @@ def test_splitk_tail_reduce_is_a_fixed_order_sum(emu, S, alpha, beta, per_row, a
     C = rng.standard_normal((N, M)).astype(np.float32)            # column-major C: rsC = 1, csC = M
     bias = rng.standard_normal(M if per_row else N).astype(np.float32) if act else None
     c0 = C.copy()
-    emu.emu_splitk_tail_reduce(p(ws), S, n_tail, n_direct, num_m, num_n, G, tile_m, M, N, alpha, beta, p(C), 1, M,
+    emu.emu_splitk_tail_reduce(p(ws), S, n_tail, n_direct, num_m, num_n, G, M, N, alpha, beta, p(C), 1, M,
                                p(bias) if bias is not None else None, per_row, act, 3)
     want = c0.T.copy()
 

@@ -44,8 +44,9 @@ def sass_counts():
 def test_tensor_core_kernels_are_wgmma_tma():
     counts = sass_counts()
     tc = {k: v for k, v in counts.items() if "gemm_tc_kernel" in k}
-    # 16-bit families (bf16, f16x3): 4 operand major-nesses x (single CTA, cluster of two); tf32 families: K-major only x 2
-    assert len(tc) == 2 * 4 * 2 + 2 * 2, sorted(tc)
+    # one-problem: 16-bit families (bf16, f16x3) x 4 operand major-nesses, tf32 families K-major only; batched: f16x3 x 4
+    # major-nesses, tf32x3, tf32x1
+    assert len(tc) == (2 * 4 + 2) + (4 + 2), sorted(tc)
     for k, c in tc.items():
         assert c["HGMMA"] >= 4 and c["WARPGROUP"] >= 2 and c["UTMALDG"] >= 2 and c["SYNCS"] >= 2, (k, dict(c))
         assert c["USETMAXREG"] == 2, k          # warp-specialised register split

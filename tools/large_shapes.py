@@ -24,7 +24,7 @@ check(100000, 3, 4096)
 check(8200, 8200, 8200)
 check(65536, 8192, 64)
 check(4096, 4096, 4096)          # split-K of the last partial wave
-check(2560, 2304, 8192)          # 90 pair-tiles: 74 direct + 16 x 4 K-ranges
+check(2560, 2304, 8192)          # 360 tiles on 132 SMs: the last wave (96) is more than half full, nothing is split
 check(20, 788544, 27)            # the im2col convolution's product as one call (AUTO: tensor cores; exact: few-rows kernel)
 check(20, 788544, 27, path=L.PATH_SIMT)
 print("ok")
