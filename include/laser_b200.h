@@ -416,6 +416,17 @@ int laser_b200_conv2d_im2col_f32_dev(float *output, const float *input, const in
                                      const float *kernel, const int64_t kshape[4], const int64_t padding[2],
                                      const int64_t strides[2], float *workspace, int64_t workspace_images,
                                      int path, void *stream);
+/* Fused convolution (the im2col prepacker of the reference's fusion roadmap, README.md:251): for every image n,
+ *   output_n <- act(conv(input_n, kernel) + bias)
+ * with input, kernel and output contiguous NCHW / [c_out][c_in][kH][kW] / NCHW device buffers and shapes, checks and
+ * results of conv2d_im2col_f32_dev.  The epilogue applies to each image's c_out x outH*outW product as in the fused GEMM
+ * entry: bias_per_row = 1 is one bias per output channel; NULL epi = no bias, no activation.  No workspace: the im2col
+ * step is folded into the preparation of the GEMM's operand, which reads the images directly, and the images of a chunk
+ * (LASER_B200_BATCH_WS_MB) share one GEMM launch.  path: as for the float32 GEMM; PATH_AUTO decides as
+ * conv2d_im2col_f32_dev does.  An unknown path or activation is EINVAL before anything is launched; n = 0 is OK. */
+int laser_b200_conv2d_f32_fused_dev(float *output, const float *input, const int64_t ishape[4],
+                                    const float *kernel, const int64_t kshape[4], const int64_t padding[2],
+                                    const int64_t strides[2], const laser_b200_epilogue *epi, int path, void *stream);
 /* host pointers, synchronous, library-owned workspace */
 int laser_b200_conv2d_im2col_f32(float *output, const float *input, const int64_t ishape[4],
                                  const float *kernel, const int64_t kshape[4], const int64_t padding[2],

@@ -374,6 +374,9 @@ struct Operand {
   // batched launch: `batch` problems s_b elements apart (the aux of their op: aux_sb apart), read through rank-3 tensor maps;
   // batch 1 with a batched launch is an operand the problems share.  0: a single problem, rank-2 maps.
   int64_t batch = 0, s_b = 0, aux_sb = 0;
+  // an im2col source: B of a convolution, [mn = outH * outW][k = C * kH * kW] per image, read from the `batch` NCHW images at
+  // ptr, s_b floats apart (s_mn, s_k unused)
+  const ConvGeom *conv = nullptr;
 };
 enum Major { K_MAJOR = 0, MN_MAJOR = 1, GENERAL = 2 };
 
@@ -559,7 +562,31 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
   });
 }
 
+// An im2col source (Operand::conv): every image's windows as K-major rows [batch][mn][ld] (split.cuh: im2col_rows_kernel) in
+// the format of `mode` -- words and fp16 pieces into hb / lb / words (F16X2), tf32 hi / lo into dst / dst_lo (TF32), the
+// values into dst (NONE: TF32X1 and the exact path)
+int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst_lo, uint16_t *hb, uint16_t *lb, int64_t ld,
+                uint32_t *words, cudaStream_t s) {
+  const Im2colSrc q = im2col_src(*o.conv);
+  const int64_t images = batch_of(o).n, rows = images * o.mn;
+  const float *in = static_cast<const float *>(o.ptr);
+  auto launch = [&](auto m) {
+    constexpr int MODE = decltype(m)::value, PER_SM = MODE == IM2COL_F16X2 ? 3 : 4;   // the kernel's launch bounds
+    if (ld <= 4 * 32 * F16ROWS_MAXV)
+      im2col_rows_kernel<MODE, 32><<<grid_for(c, (rows + 7) / 8, PER_SM), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb, ld, words);
+    else
+      im2col_rows_kernel<MODE, 256><<<grid_for(c, rows, PER_SM), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb, ld, words);
+  };
+  if (mode == SPLIT_F16X2) launch(std::integral_constant<int, IM2COL_F16X2>());
+  else if (mode == SPLIT_TF32) launch(std::integral_constant<int, IM2COL_TF32>());
+  else launch(std::integral_constant<int, IM2COL_F32>());
+  COUNT_LAUNCH();
+  CHECK_LAUNCH();
+  return LASER_B200_OK;
+}
+
 // One operand of a tensor-core call: first the plan, then its steps.
+//   An im2col source: one pass from the images into the prepared rows, K-major like a gathered operand.
 //   bf16 K- or MN-major; TF32X1 K-major without op: TMA reads the caller's memory, no workspace.
 //   TF32X3 K-major; F16X3 K- or MN-major -- without op, or with aux laid out like the operand: the split reads the caller's
 //     memory and applies the op on load (F16X3 MN-major: all column scales first, then the split).
@@ -572,12 +599,13 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
 template <int ESZ>
 int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w, int block_mn,
                     OperandMaps *m, bool *used_ws, cudaStream_t s, const OperandOp *op = nullptr) {
-  const Major mj = classify(o, ESZ);
+  const bool conv = o.conv != nullptr;   // (fp32, no op)
+  const Major mj = conv ? K_MAJOR : classify(o, ESZ);
   const Batch bt = batch_of(o);
   const bool rows_ok = bt.n == 1 || ((o.s_b * ESZ) % 16 == 0 && (!op || !op->aux || o.aux_sb % 4 == 0));
   const bool map_ok = bt.n == 1 || (o.s_b > 0 && o.s_b < (static_cast<int64_t>(1) << 40) / ESZ);
   const bool tma_layout = (mj == K_MAJOR || (mj == MN_MAJOR && (ESZ == 2 || mode == SPLIT_F16X2))) && rows_ok;
-  const bool in_place = tma_layout && (mode == SPLIT_NONE ? !op && map_ok : !op || op_same_layout(o, *op));
+  const bool in_place = !conv && tma_layout && (mode == SPLIT_NONE ? !op && map_ok : !op || op_same_layout(o, *op));
   const Major out_mj = in_place ? mj : K_MAJOR;              // layout of the arrays the tensor-core kernel reads
   const int64_t R = (out_mj == K_MAJOR) ? o.mn : o.k;        // their rows
   const int64_t Cc = (out_mj == K_MAJOR) ? o.k : o.mn;       // their contiguous extent
@@ -609,7 +637,9 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
         return set_error(LASER_B200_ECUDA, "internal: F16X3 scale buffer not sized for this operand");
       uint16_t *hb = static_cast<uint16_t *>(w.p0->ptr), *lb = static_cast<uint16_t *>(w.p1->ptr);
       uint32_t *words = static_cast<uint32_t *>(c.f16s.ptr) + w.amax_off;
-      if (!in_place) {   // the gathered problems are stacked rows: one plain row pass over all of them
+      if (conv) {
+        rc = im2col_rows(c, o, mode, nullptr, nullptr, hb, lb, ld_b, words, s);
+      } else if (!in_place) {   // the gathered problems are stacked rows: one plain row pass over all of them
         if ((rc = gather<float>(c, o, *w.gather, nullptr, s, op))) return rc;
         rc = f16x2_rows(c, static_cast<const float *>(w.gather->ptr), bt.n * R, Cc, ld, hb, lb, ld_b, words, s);
       } else if (out_mj == K_MAJOR) {
@@ -622,13 +652,15 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
       if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, o.k, ld_b, block_mn, depth, d_stride(ld_b)))) return rc;
       return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, o.k, ld_b, block_mn, depth, d_stride(ld_b));
     }
-    if (!in_place) {
+    if (!in_place && !conv) {
       rc = (mode == SPLIT_TF32) ? gather<float, 1>(c, o, *w.p0, w.p1, s, op) : gather<float>(c, o, *w.p0, nullptr, s, op);
-    } else {   // TF32X3, K-major
+    } else {   // TF32X3 K-major, or an im2col source (TF32X3, TF32X1)
       const size_t bytes = static_cast<size_t>(bt.n * R) * ld * sizeof(float);
       if ((rc = ensure(*w.p0, bytes))) return rc;
-      if ((rc = ensure(*w.p1, bytes))) return rc;
-      rc = tf32_split(c, src, R, Cc, src_ld, static_cast<float *>(w.p0->ptr), static_cast<float *>(w.p1->ptr), ld, s, on_load, bt);
+      if (mode == SPLIT_TF32 && (rc = ensure(*w.p1, bytes))) return rc;
+      float *p0 = static_cast<float *>(w.p0->ptr), *p1 = mode == SPLIT_TF32 ? static_cast<float *>(w.p1->ptr) : nullptr;
+      rc = conv ? im2col_rows(c, o, mode, p0, p1, nullptr, nullptr, ld, nullptr, s)
+                : tf32_split(c, src, R, Cc, src_ld, p0, p1, ld, s, on_load, bt);
     }
     if (rc) return rc;
   }
@@ -747,10 +779,11 @@ template <int SRC_ESZ, typename OutT>
 int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, const void *A, int64_t rsA,
             int64_t csA, const void *B, int64_t rsB, int64_t csB, float beta, OutT *C, int64_t rsC,
             int64_t csC, cudaStream_t s, const Epilogue &epi, cudaEvent_t b_ready = nullptr, const OperandOp *opA = nullptr,
-            const OperandOp *opB = nullptr, const BatchArgs *bat = nullptr) {
+            const OperandOp *opB = nullptr, const BatchArgs *bat = nullptr, const ConvGeom *convB = nullptr) {
   // b_ready: B becomes valid only when this event has fired (the row-sharded driver: B is in flight on the communication
   // stream); everything that does not read B -- the preparation of A -- is queued before the wait.
   // opA / opB: operand ops applied while the operands are prepared (fp32 only)
+  // convB: B is an im2col source, the images at B (batched: bat->B floats apart; rsB, csB unused)
   if (M > 0x7fffffffLL || N > 0x7fffffffLL || K > 0x7fffffffLL)
     return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: extents must fit in int32");
   std::lock_guard<std::mutex> lk(c.mu);  // workspace + descriptor construction are per context
@@ -764,6 +797,7 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
     oa.batch = a_shared ? 1 : bat->batch; oa.s_b = bat->A; oa.aux_sb = bat->auxA;
     ob.batch = b_shared ? 1 : bat->batch; ob.s_b = bat->B; ob.aux_sb = bat->auxB;
   }
+  ob.conv = convB;
   OperandMaps ma, mb;
   bool used_ws = false;
   // the previous call may still be reading the workspace on another stream
@@ -1183,6 +1217,74 @@ int batched_fused_entry(int64_t batch, int64_t M, int64_t N, int64_t K, float al
   if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
   if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
   return batched_fused_dev(batch, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, bs, pa, pb, e, path, stream);
+}
+
+// ---------------------------------------------------------------------------------------
+//     fused convolution: im2col folded into the preparation of B, the images of a chunk in one GEMM launch
+// ---------------------------------------------------------------------------------------
+// Exact path, `images` images: their windows as plain K-major rows in the gather workspace, one batched exact-kernel launch
+int conv2d_simt(Ctx &c, const ConvGeom &g, int64_t images, const float *kernel, const float *input, float *output, cudaStream_t s,
+                const Epilogue &epi) {
+  const int64_t M = g.Cout, K = g.K(), N = g.outHW(), ld = round_up(K, 4);
+  std::lock_guard<std::mutex> lk(c.mu);   // the gather buffer is workspace
+  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
+  int rc;
+  if ((rc = ensure(c.gather[1], static_cast<size_t>(images * N) * ld * sizeof(float)))) return rc;
+  Operand o{input, N, K, 0, 0, images, g.C * g.H * g.W};
+  o.conv = &g;
+  float *rows = static_cast<float *>(c.gather[1].ptr);
+  if ((rc = im2col_rows(c, o, SPLIT_NONE, rows, nullptr, nullptr, nullptr, ld, nullptr, s))) return rc;
+  if ((rc = gemm_simt<float>(c, M, N, K, 1.0f, kernel, K, 1, rows, 1, ld, 0.0f, output, N, 1, s, epi, images, 0, N * ld, M * N)))
+    return rc;
+  CUDA_TRY(cudaEventRecord(c.ws_free, s));
+  return LASER_B200_OK;
+}
+
+// laser_b200_conv2d_f32_fused_dev (capi_layers.inc checks the geometry): output_n = act(F * im2col(input_n) + bias) for every
+// image n.  A = the filters F [Cout][K], shared by the images (prepared once per launch); B = the images as an im2col source.
+int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const float *kernel, const laser_b200_epilogue *epi_in,
+                     int path, void *stream) {
+  Epilogue epi;
+  int rc;
+  if ((rc = epilogue_of(epi_in, &epi))) return rc;
+  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
+    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  if (g.B == 0) return LASER_B200_OK;
+  if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
+  const int64_t M = g.Cout, K = g.K(), N = g.outHW(), image = g.C * g.H * g.W;
+  // PATH_AUTO decides as conv2d_im2col_f32_dev does: the exact kernel for a batch of short M or K (batched_f32_dev), else
+  // resolve_auto with this call's epilogue (never the GEMV: N is a pixel count and the batch needs one launch)
+  if (path == LASER_B200_PATH_AUTO)
+    path = (g.B > 1 && (M < 64 || K < 64)) ? LASER_B200_PATH_SIMT : resolve_auto(M, N, K, epi, /*operand_op=*/true);
+  if (g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0) {   // the image already is the [C][H*W] matrix
+    const laser_b200_batch_strides bs{0, image, M * N, 0, 0};
+    return batched_fused_dev(g.B, M, N, K, 1.0f, kernel, K, 1, input, N, 1, 0.0f, output, N, 1, &bs, nullptr, nullptr, epi, path,
+                             stream);
+  }
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  // chunks of whole images, as batched_fused_dev makes them (the exact path's rows count as an op'd B)
+  const int64_t per = batch_ws_per_problem(path, M, N, K, false, true, false, true);
+  int64_t chunk = c->batch_ws_bytes / per;
+  const int64_t tiles = ((M + TC_BLOCK_M - 1) / TC_BLOCK_M) * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N);
+  if (chunk > 0x7fffffffLL / (16 * tiles)) chunk = 0x7fffffffLL / (16 * tiles);
+  if (chunk < 1) chunk = 1;
+  for (int64_t n0 = 0; n0 < g.B; n0 += chunk) {
+    const int64_t cnt = g.B - n0 < chunk ? g.B - n0 : chunk;
+    const float *in = input + n0 * image;
+    float *out = output + n0 * M * N;
+    if (path == LASER_B200_PATH_SIMT) {
+      rc = conv2d_simt(*c, g, cnt, kernel, in, out, s, epi);
+    } else {
+      const BatchArgs bat{cnt, 0, image, M * N, 0, 0};
+      rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, 1.0f, kernel, K, 1, in, 0, 0, 0.0f, out, N, 1, s, epi, nullptr, nullptr,
+                             nullptr, &bat, &g);
+    }
+    if (rc) return rc;
+  }
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1709,5 +1811,6 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 }  // extern "C"
 
 #define LB200_BATCHED_FUSED_F32 batched_fused_entry
+#define LB200_CONV2D_FUSED_F32 conv2d_fused_dev
 #include "capi_layers.inc"
 #include "capi_multi.inc"

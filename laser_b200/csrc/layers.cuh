@@ -83,6 +83,13 @@ transpose_batched_kernel(T *__restrict__ dst, const T *__restrict__ src, int64_t
   }
 }
 
+// ---- convolution geometry (conv2d_common.nim:6-45): NCHW images, [Cout][C][kH][kW] filters ----
+struct ConvGeom {
+  int64_t B, C, H, W, Cout, kH, kW, pH, pW, sH, sW, outH, outW;
+  __host__ __device__ int64_t K() const { return C * kH * kW; }
+  __host__ __device__ int64_t outHW() const { return outH * outW; }
+};
+
 // ---- im2col: images x [C][H][W] -> images x [C*kH*kW][outH*outW], zero outside the image ----
 struct Im2colParams {
   int C, H, W, kH, kW, pH, pW, sH, sW, outH, outW;

@@ -18,6 +18,7 @@
 #include <stdint.h>
 
 #include "f16_scale.cuh"
+#include "layers.cuh"
 #include "ptx.cuh"
 #include "tc_params.h"
 
@@ -454,6 +455,120 @@ split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
       if constexpr (HAS_OP) v = op_vec(o, v, r, c, Cc);
       if constexpr (!PER_COL) sx = sy = sz = sw = f16x2_scale(absmax_b[r]);
       store_f16x2_vec4(v, sx, sy, sz, sw, hb_b + r * ld_b, lb_b + r * ld_b, c);
+    }
+  }
+}
+
+// ---- im2col source: a convolution's B operand prepared straight from the NCHW images ---------------------------------
+// Row n * outHW + p -- image n of the launch, output pixel p = oh * outW + ow -- is the pixel's receptive field in the
+// reference's im2col order k = (c * kH + krow) * kW + kcol (conv2d_im2col.nim:69-93), 0 where the window leaves the padded
+// image: the im2col matrix transposed, K-major, stacked [images][outHW][ld] like a gathered batched operand.  Each row is
+// written in the format of the preparation step it replaces, bit for bit:
+//   IM2COL_F32   the values, ld = round_up(K, 4)                                (TF32X1, exact path)
+//   IM2COL_TF32  hi / lo pieces as split_rows_tf32_kernel, ld = round_up(K, 4)  (TF32X3)
+//   IM2COL_F16X2 abs-max word + both fp16 pieces as f16x2_rows_fused_kernel, ld = round_up(K, 8)  (F16X3): one pass, the row
+//                held in registers (F16ROWS_MAXV float4 per thread) while its abs-max is reduced
+// Every column up to ld is written (zeros past K).  The window is read with plain cached loads: the 256 / GROUP rows of a
+// CTA are neighbouring pixels, whose windows overlap, and the image is small enough to stay in L2 between CTAs.
+// GROUP: a warp per row (ld <= 1024), the CTA per row otherwise (the part of the row past the registers is read twice).
+enum Im2colMode { IM2COL_F32 = 0, IM2COL_TF32 = 1, IM2COL_F16X2 = 2 };
+struct Im2colSrc {   // int32 geometry of one launch (conv_geom bounds K, outHW and H * W by 2^31)
+  int C, H, W, kH, kW, pH, pW, sH, sW, outW, K;
+  int64_t outHW, image;   // pixels per image, floats per input image
+};
+inline Im2colSrc im2col_src(const ConvGeom &g) {
+  return Im2colSrc{static_cast<int>(g.C), static_cast<int>(g.H), static_cast<int>(g.W), static_cast<int>(g.kH),
+                   static_cast<int>(g.kW), static_cast<int>(g.pH), static_cast<int>(g.pW), static_cast<int>(g.sH),
+                   static_cast<int>(g.sW), static_cast<int>(g.outW), static_cast<int>(g.K()), g.outHW(), g.C * g.H * g.W};
+}
+// elements k .. k+3 of the window of output pixel (oh, ow) of image `img` (0 past K)
+__device__ __forceinline__ float4 window_vec(const float *__restrict__ img, const Im2colSrc &q, int oh, int ow, int k) {
+  const int khw = q.kH * q.kW;
+  int c = k / khw;
+  int kr = (k - c * khw) / q.kW;
+  int kc = k - c * khw - kr * q.kW;
+  float v[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const int h = oh * q.sH - q.pH + kr, w = ow * q.sW - q.pW + kc;
+    const bool inside = k + e < q.K && static_cast<unsigned>(h) < static_cast<unsigned>(q.H) &&
+                        static_cast<unsigned>(w) < static_cast<unsigned>(q.W);
+    v[e] = inside ? img[(static_cast<int64_t>(c) * q.H + h) * q.W + w] : 0.0f;
+    if (++kc == q.kW) { kc = 0; if (++kr == q.kH) { kr = 0; ++c; } }
+  }
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+// (F16X2: the row in registers next to the geometry needs more than the 64 registers of 4 CTAs per SM -- it spills there)
+template <int MODE, int GROUP>
+__global__ void __launch_bounds__(256, MODE == IM2COL_F16X2 ? 3 : 4)
+im2col_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, float *__restrict__ dst, float *__restrict__ dst_lo,
+                   uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld, uint32_t *__restrict__ absmax) {
+  static_assert(GROUP == 32 || GROUP == 256, "a warp or the CTA per row");
+  __shared__ uint32_t red[2][8];
+  ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
+  const int tid = static_cast<int>(threadIdx.x) % GROUP;
+  const int64_t per_cta = 256 / GROUP;
+  const int64_t first = static_cast<int64_t>(blockIdx.x) * per_cta + static_cast<int64_t>(threadIdx.x) / GROUP;
+  const int64_t step = static_cast<int64_t>(gridDim.x) * per_cta;
+  const int nvec = static_cast<int>(ld >> 2);   // float4 groups written per row, padding included
+  int parity = 0;
+  // GROUP == 256: every thread of the CTA runs the same number of iterations (the loop holds a __syncthreads)
+  for (int64_t r = first; r < images * q.outHW; r += step) {
+    const int64_t n = r / q.outHW;
+    const int p = static_cast<int>(r - n * q.outHW);
+    const int oh = p / q.outW, ow = p - oh * q.outW;
+    const float *img = in + n * q.image;
+    if constexpr (MODE != IM2COL_F16X2) {
+      for (int idx = tid; idx < nvec; idx += GROUP) {
+        const float4 v = window_vec(img, q, oh, ow, idx << 2);
+        if constexpr (MODE == IM2COL_F32) {
+          *reinterpret_cast<float4 *>(dst + r * ld + (idx << 2)) = v;
+        } else {
+          float4 h, l;
+          h.x = tf32_rna(v.x); l.x = tf32_lo(v.x, h.x);
+          h.y = tf32_rna(v.y); l.y = tf32_lo(v.y, h.y);
+          h.z = tf32_rna(v.z); l.z = tf32_lo(v.z, h.z);
+          h.w = tf32_rna(v.w); l.w = tf32_lo(v.w, h.w);
+          *reinterpret_cast<float4 *>(dst + r * ld + (idx << 2)) = h;
+          *reinterpret_cast<float4 *>(dst_lo + r * ld + (idx << 2)) = l;
+        }
+      }
+    } else {
+      float4 v[F16ROWS_MAXV];
+      uint32_t m = 0u;
+#pragma unroll
+      for (int i = 0; i < F16ROWS_MAXV; ++i) {
+        const int idx = tid + i * GROUP;
+        if (idx < nvec) {
+          v[i] = window_vec(img, q, oh, ow, idx << 2);
+          m = max(max(m, finite_abs_bits(v[i].x)), max(finite_abs_bits(v[i].y), max(finite_abs_bits(v[i].z), finite_abs_bits(v[i].w))));
+        }
+      }
+      for (int idx = tid + F16ROWS_MAXV * GROUP; idx < nvec; idx += GROUP) {
+        const float4 t = window_vec(img, q, oh, ow, idx << 2);
+        m = max(max(m, finite_abs_bits(t.x)), max(finite_abs_bits(t.y), max(finite_abs_bits(t.z), finite_abs_bits(t.w))));
+      }
+      float mf = __uint_as_float(m);     // non-negative finite: fmaxf orders them like the integers
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mf = fmaxf(mf, __shfl_xor_sync(0xffffffffu, mf, o));
+      m = __float_as_uint(mf);
+      if constexpr (GROUP == 256) {
+        if ((threadIdx.x & 31) == 0) red[parity][threadIdx.x >> 5] = m;
+        __syncthreads();
+#pragma unroll
+        for (int w = 0; w < 8; ++w) m = max(m, red[parity][w]);
+        parity ^= 1;   // the next row uses the other buffer: one barrier per row is enough
+      }
+      if (tid == 0) absmax[r] = m;
+      const float s = f16x2_scale(m);
+      uint16_t *hrow = hb + r * ld, *lrow = lb + r * ld;
+#pragma unroll
+      for (int i = 0; i < F16ROWS_MAXV; ++i) {
+        const int idx = tid + i * GROUP;
+        if (idx < nvec) store_f16x2_vec(v[i], s, hrow, lrow, static_cast<int64_t>(idx) << 2);
+      }
+      for (int idx = tid + F16ROWS_MAXV * GROUP; idx < nvec; idx += GROUP)
+        store_f16x2_vec(window_vec(img, q, oh, ow, idx << 2), s, hrow, lrow, static_cast<int64_t>(idx) << 2);
     }
   }
 }

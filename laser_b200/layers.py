@@ -7,6 +7,8 @@
     conv2d_out_shape, im2col_workspace_size       benchmarks/convolution/conv2d_common.nim:15-45,
                                                   conv2d_im2col.nim:8-18
     im2col, conv2d_im2col                         conv2d_im2col.nim:44-166
+    conv2d_fused                                  conv2d_im2col.nim:95-166 + bias + activation, im2col folded into the
+                                                  GEMM's operand preparation (README.md:251)
     gemm_strided_batched                          (roadmap item of the reference, README.md:253-263)
     copyFrom(dst, src)                            laser/tensor/initialization.nim:80-112
 
@@ -17,14 +19,14 @@ import ctypes
 
 import numpy as np
 
-from ._capi import PATH_AUTO, check, lib
+from ._capi import PATH_AUTO, Epilogue, check, lib
 from .gemm import _current_stream, _resolve, _scalar
 from .tensor import _ITEMSIZE, Tensor
 
 FOREACH_OPS = {"copy": 0, "fill": 1, "scale": 2, "add": 3, "sub": 4, "mul": 5, "fma": 6, "axpy": 7, "bench": 8}
 
 __all__ = ["forEach", "FOREACH_OPS", "transpose2D_copy", "transpose2D_batched", "nchw2nhwc", "nhwc2nchw", "conv2d_out_shape",
-           "im2col_workspace_size", "im2col", "conv2d_im2col", "gemm_strided_batched", "copyFrom"]
+           "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "gemm_strided_batched", "copyFrom"]
 
 _i64 = ctypes.c_int64
 
@@ -126,6 +128,22 @@ def conv2d_im2col(output, input, ishape, kernel, kshape, padding, strides, works
     pw = _dev_f32(workspace) if workspace is not None else 0
     check(lib().laser_b200_conv2d_im2col_f32_dev(po, pi, _i4(ishape), pk, _i4(kshape), _i2(padding), _i2(strides), pw,
                                                  int(workspace_images), int(path), stream))
+
+
+def conv2d_fused(output, input, ishape, kernel, kshape, padding, strides, bias=None, bias_per_row=True, activation="none",
+                 path=PATH_AUTO, stream=None):
+    """output_n <- act(conv(input_n, kernel) + bias) for every image n, on float32 DEVICE buffers (NCHW in and out, kernel
+    [c_out, c_in, kH, kW]).  bias_per_row=True: one bias per output channel.  activation: none | relu | tanh | sigmoid.
+    The im2col step is folded into the preparation of the GEMM operand: no workspace, one GEMM launch for the images."""
+    po, pi, pk = _dev_f32(output), _dev_f32(input), _dev_f32(kernel)
+    epi = Epilogue()
+    if bias is not None:
+        epi.bias = _dev_f32(bias)
+    epi.bias_per_row = 1 if bias_per_row else 0
+    epi.activation = {"none": 0, "relu": 1, "tanh": 2, "sigmoid": 3}[activation]
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_f32_fused_dev(po, pi, _i4(ishape), pk, _i4(kshape), _i2(padding), _i2(strides),
+                                                ctypes.byref(epi), int(path), stream))
 
 
 def gemm_strided_batched(batch, M, N, K, alpha, A, rowStrideA, colStrideA, batchStrideA, B, rowStrideB, colStrideB,

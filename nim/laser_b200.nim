@@ -276,6 +276,10 @@ proc laser_b200_conv2d_out_shape*(ishape, kshape: ptr array[4, int64], padding, 
                                   oshape: ptr array[4, int64]): cint
 proc laser_b200_conv2d_im2col_f32*(output, input: ptr float32, ishape: ptr array[4, int64], kernel: ptr float32,
                                    kshape: ptr array[4, int64], padding, strides: ptr array[2, int64]): cint
+# fused convolution on device buffers (README.md:251): output_n <- act(conv(input_n, kernel) + bias); nil epi = none
+proc laser_b200_conv2d_f32_fused_dev*(output, input: ptr float32, ishape: ptr array[4, int64], kernel: ptr float32,
+                                      kshape: ptr array[4, int64], padding, strides: ptr array[2, int64],
+                                      epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
 {.pop.}
 
 proc transpose2D_copy*[T](dst, src: ptr (T or UncheckedArray[T]), NR, NC: Natural) =
