@@ -136,6 +136,24 @@ static int dispatch(int a_mn, int b_mn, const Args &a_in) {
 #undef GO
 }
 
+// the library's launch plan alone (tc_plan, as capi.cu: tc_run calls it) of `batch` problems of M x N x K on `sm_count` SMs:
+// out = {k_splits, n_direct}.  kind as below.
+extern "C" void emu_tc_plan(int kind, int64_t M, int64_t N, int64_t K, int batch, int kc_faithful, int splitk_enabled, int sm_count,
+                            int tail_min_k, int *out) {
+  TcParams p;
+  p.M = M; p.N = N; p.K = K; p.batch = batch;
+  TcPlanCfg cfg{kc_faithful, 0, splitk_enabled != 0, sm_count};
+  if (tail_min_k > 0) cfg.tail_min_k = tail_min_k;
+  switch (kind) {
+    case 0: tc_plan<4, true>(p, 1, cfg); break;
+    case 1: tc_plan<4, true>(p, 3, cfg); break;
+    case 2: tc_plan<2, false>(p, 1, cfg); break;
+    default: tc_plan<2, true>(p, 3, cfg); break;
+  }
+  out[0] = p.k_splits;
+  out[1] = p.n_direct;
+}
+
 // kind: 0 tf32x1, 1 tf32x3, 2 bf16, 3 f16x3 (tc_launch.h: the four kernel families)
 extern "C" int emu_gemm_tc(int kind, int a_mn, int b_mn, int64_t M, int64_t N, int64_t K, float alpha, float beta,
                            const void *A0, const void *A1, int64_t ldA, const void *B0, const void *B1, int64_t ldB,
