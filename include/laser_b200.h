@@ -232,6 +232,32 @@ int laser_b200_gemm_strided_batched_f32_fused_dev(int64_t batch, int64_t M, int6
                                                   const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
                                                   const laser_b200_epilogue *epi, int path, void *stream);
 
+/* ---- batch-reduced fused product -----------------------------------------
+ * The sum of a batch's products into one C (torch.addbmm, einsum 'bmk,bkn->mn'):
+ *   C <- act(alpha * sum_b opA(A_b) * opB(B_b) + beta * C + bias),   X_b = X + b * batchStrides->X
+ * for A, B and the aux tensors of opA / opB.  It is the weight gradient of a batched layer, and the filter gradient of a
+ * convolution over channel-first data, where the batch does not collapse into one long K of a plain fused call.  The call is
+ * one fused product over the operands concatenated along K, A^ = [opA(A_0) | .. | opA(A_{batch-1})] (M x batch*K) and
+ * B^ = [opB(B_0); ..; opB(B_{batch-1})] (batch*K x N): the operand preparation writes the concatenation, and one GEMM launch
+ * (split along K like any long product) computes it.  C is bit for bit what laser_b200_gemm_strided_f32_fused_dev gives over
+ * materialised A^ and B^ on the same path, and the activation is applied once, to the whole sum.
+ *   Strides are in elements and may be negative.  A stride of 0 repeats A (or B) in every K segment: it is prepared batch
+ *   times, like distinct operands.  batchStrides->C must be 0: there is one C.
+ *   PATH_AUTO takes the path of a fused call with an op over A^ and B^ (it never takes the N <= 4 GEMV shortcut).
+ *   batch == 1 is exactly laser_b200_gemm_strided_f32_fused_dev.  batch == 0, or M, N or K == 0: LASER_B200_OK, nothing is
+ *   launched and C is untouched.  batch * K must fit in int32 on the tensor-core paths (LASER_B200_EUNSUPPORTED otherwise).
+ *   LASER_B200_EINVAL, before anything is launched: batch < 0; batchStrides == NULL with batch > 0; batchStrides->C != 0;
+ *   an unknown op, or a derivative op without aux; an unknown path.
+ *   The whole batch runs as one chunk, whatever LASER_B200_BATCH_WS_MB says: chunks would round C between them and apply the
+ *   activation to a partial sum.  The workspace is that of the fused call over A^ and B^. */
+int laser_b200_gemm_strided_batch_reduce_f32_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha,
+                                                       const float *A, int64_t rowStrideA, int64_t colStrideA,
+                                                       const float *B, int64_t rowStrideB, int64_t colStrideB,
+                                                       float beta, float *C, int64_t rowStrideC, int64_t colStrideC,
+                                                       const laser_b200_batch_strides *batchStrides,
+                                                       const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
+                                                       const laser_b200_epilogue *epi, int path, void *stream);
+
 /* ---- pre-packed operands (device) -----------------------------------------
  * Replaces  gemm_prepackA_mem_required / gemm_prepackB_mem_required, gemm_prepackA / gemm_prepackB
  * and gemm_packed   (laser/primitives/matrix_multiplication/gemm_prepacked.nim:63-292).

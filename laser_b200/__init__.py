@@ -6,8 +6,8 @@ host-side mirror of the reference interface on top of it.  See DESIGN.md / INTEG
 """
 from ._capi import (PATH_AUTO, PATH_BF16, PATH_F16X3, PATH_NAMES, PATH_SIMT, PATH_TF32X1, PATH_TF32X3, LaserB200Error, lib,
                     lib_path)
-from .gemm import (DevPtr, fill_uniform_f32, gemm_strided, gemm_strided_batched_fused, gemm_strided_fused, get_f32_mode, init,
-                   last_path,
+from .gemm import (DevPtr, fill_uniform_f32, gemm_strided, gemm_strided_batch_reduce_fused, gemm_strided_batched_fused,
+                   gemm_strided_fused, get_f32_mode, init, last_path,
                    launch_count, profile_begin, profile_end, set_f32_mode, shutdown,
                    synchronize)
 from .layers import (FOREACH_OPS, conv2d_fused, conv2d_im2col, conv2d_out_shape, copyFrom, forEach, gemm_strided_batched, im2col,

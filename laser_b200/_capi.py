@@ -74,6 +74,8 @@ SIGNATURES = {
                                                                               ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
     "laser_b200_gemm_strided_batched_f32_fused_dev": (ctypes.c_int, [i64] + _gemm_sig(f32) + [
         ctypes.POINTER(BatchStrides), ctypes.POINTER(OperandOp), ctypes.POINTER(OperandOp), ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
+    "laser_b200_gemm_strided_batch_reduce_f32_fused_dev": (ctypes.c_int, [i64] + _gemm_sig(f32) + [
+        ctypes.POINTER(BatchStrides), ctypes.POINTER(OperandOp), ctypes.POINTER(OperandOp), ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
     "laser_b200_gemm_strided_f64_dev": (ctypes.c_int, _gemm_sig(f64) + [vp]),
     "laser_b200_gemm_strided_i32_dev": (ctypes.c_int, _gemm_sig(i32) + [vp]),
     "laser_b200_gemm_strided_i64_dev": (ctypes.c_int, _gemm_sig(i64) + [vp]),

@@ -377,6 +377,9 @@ struct Operand {
   // an im2col source: B of a convolution, [mn = outH * outW][k = C * kH * kW] per image, read from the `batch` NCHW images at
   // ptr, s_b floats apart (s_mn, s_k unused)
   const ConvGeom *conv = nullptr;
+  // a concatenated batch: the operand of a sum of products, [mn][batch * k], whose k-segment b is problem b's [mn][k] (s_b
+  // apart, 0: the same matrix in every segment); prepared into compact workspace and read through rank-2 maps
+  bool concat = false;
 };
 enum Major { K_MAJOR = 0, MN_MAJOR = 1, GENERAL = 2 };
 
@@ -466,16 +469,18 @@ inline bool op_same_layout(const Operand &o, const OperandOp &op) {
 
 // ---- the preparation steps: one function, and one launch site, per kernel family of split.cuh ----
 // A step takes its op as a pointer (nullptr: none) and its problems as a Batch (n == 1: one problem), and hands `launch`
-// (has_op, op, batched): has_op is std::true_type with *op or std::false_type with OperandOp(), batched is std::true_type
-// when bt.n > 1.  The kernel's plain, HAS_OP and BATCHED instantiations come from the same launch statement.
+// (has_op, op, batched, concat): has_op is std::true_type with *op or std::false_type with OperandOp(), batched is
+// std::true_type when bt.n > 1, concat std::true_type for a concatenated batch (Operand::concat, with batched).  The kernel's
+// plain, HAS_OP, BATCHED and CONCAT instantiations come from the same launch statement.
 template <typename Launch>
-int launch_prep(const OperandOp *op, const Batch &bt, Launch launch) {
-  auto with_op = [&](auto batched) {
-    if (op) launch(std::true_type(), *op, batched);
-    else launch(std::false_type(), OperandOp(), batched);
+int launch_prep(const OperandOp *op, const Batch &bt, Launch launch, bool concat = false) {
+  auto with_op = [&](auto batched, auto cat) {
+    if (op) launch(std::true_type(), *op, batched, cat);
+    else launch(std::false_type(), OperandOp(), batched, cat);
   };
-  if (bt.n > 1) with_op(std::true_type());
-  else with_op(std::false_type());
+  if (concat) with_op(std::true_type(), std::true_type());
+  else if (bt.n > 1) with_op(std::true_type(), std::false_type());
+  else with_op(std::false_type(), std::false_type());
   COUNT_LAUNCH();
   CHECK_LAUNCH();
   return LASER_B200_OK;
@@ -486,80 +491,87 @@ inline Batch batch_of(const Operand &o) { return Batch{o.batch > 1 ? o.batch : 1
 // The gather: op(operand), or the operand itself, from any strides into compact K-major rows [mn][round_up(k, 16 / sizeof(T))]
 // allocated in dst (aux read with its own strides).  MODE 1 (fp32): the tf32 hi / lo pieces into dst / *lo.  bf16 operands
 // carry no op.
-// A batched operand: the problems' rows stacked, [batch][mn][ld].
+// A batched operand: the problems' rows stacked, [batch][mn][ld]; a concatenated one: [mn][round_up(batch * k, ..)].
 template <typename T, int MODE = 0>
 int gather(Ctx &c, const Operand &o, Buffer &dst, Buffer *lo, cudaStream_t s, const OperandOp *op = nullptr) {
   const Batch bt = batch_of(o);
-  const int64_t ld = round_up(o.k, 16 / static_cast<int64_t>(sizeof(T)));
-  const size_t bytes = static_cast<size_t>(bt.n * o.mn) * ld * sizeof(T);
+  const int64_t ld = round_up(o.concat ? bt.n * o.k : o.k, 16 / static_cast<int64_t>(sizeof(T)));
+  const size_t bytes = static_cast<size_t>((o.concat ? 1 : bt.n) * o.mn) * ld * sizeof(T);
   int rc;
   if ((rc = ensure(dst, bytes))) return rc;
   if (MODE == 1 && (rc = ensure(*lo, bytes))) return rc;
   const int64_t tiles = ((o.mn + 31) / 32) * ((o.k + 31) / 32) * bt.n;
   const int read_along_r = (llabs(o.s_mn) < llabs(o.s_k)) ? 1 : 0;
   T *d0 = static_cast<T *>(dst.ptr), *d1 = MODE == 1 ? static_cast<T *>(lo->ptr) : nullptr;
-  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
-    constexpr bool HAS_OP = decltype(has_op)::value && sizeof(T) == 4, BATCHED = decltype(batched)::value && sizeof(T) == 4;
-    pack_general_kernel<T, MODE, HAS_OP, BATCHED><<<grid_for(c, tiles, 8), 256, 0, s>>>(
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched, auto cat) {
+    constexpr bool HAS_OP = decltype(has_op)::value && sizeof(T) == 4, BATCHED = decltype(batched)::value && sizeof(T) == 4,
+                   CONCAT = decltype(cat)::value && sizeof(T) == 4;
+    pack_general_kernel<T, MODE, HAS_OP, BATCHED, CONCAT><<<grid_for(c, tiles, 8), 256, 0, s>>>(
         static_cast<const T *>(o.ptr), o.mn, o.k, o.s_mn, o.s_k, d0, d1, ld, read_along_r, k, bt);
-  });
+  }, o.concat);
 }
 
-// TF32X3 in place: tf32 hi / lo pieces [R][ld] of fp32 rows [R][Cc], src_ld apart
+// TF32X3 in place: tf32 hi / lo pieces [R][ld] of fp32 rows [R][Cc], src_ld apart (concat: of the batch's rows laid end to
+// end, [R][bt.n * Cc])
 int tf32_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, float *hi, float *lo, int64_t ld, cudaStream_t s,
-               const OperandOp *op, const Batch &bt = Batch()) {
-  const int64_t items = bt.n * R * ((Cc + 3) / 4);
-  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
-    split_rows_tf32_kernel<decltype(has_op)::value, decltype(batched)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
-        src, R, Cc, src_ld, hi, lo, ld, k, bt);
-  });
+               const OperandOp *op, const Batch &bt = Batch(), bool concat = false) {
+  const int64_t items = concat ? R * ((bt.n * Cc + 3) / 4) : bt.n * R * ((Cc + 3) / 4);
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched, auto cat) {
+    constexpr bool HAS_OP = decltype(has_op)::value, BATCHED = decltype(batched)::value, CONCAT = decltype(cat)::value;
+    split_rows_tf32_kernel<HAS_OP, BATCHED, CONCAT><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(src, R, Cc, src_ld, hi, lo,
+                                                                                                       ld, k, bt);
+  }, concat);
 }
 
 // F16X3, one scale per row of fp32 rows [R][Cc] (src_ld apart): the abs-max word of each row, the scale and the two fp16
 // pieces [R][ld_b] in ONE pass (split.cuh).  Rows of up to 1024 floats: a warp per row.  Longer rows: prefetched into a
 // shared-memory ring by the copy engine when they allow it (16-byte aligned, at most 8192 floats; the ring kernel has no op
-// variant, nor a batched one), the CTA per row otherwise.
+// variant, nor a batched one), the CTA per row otherwise.  concat: the batch's rows laid end to end, rows of bt.n * Cc floats.
 int f16x2_rows(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *hb, uint16_t *lb, int64_t ld_b,
-               uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr, const Batch &bt = Batch()) {
+               uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr, const Batch &bt = Batch(), bool concat = false) {
   const bool ring = !op && bt.n == 1 && f16x2_rows_ring_ok(src, Cc, src_ld);
   if (ring && !c.ring_attr_set) {
     CUDA_TRY(cudaFuncSetAttribute(f16x2_rows_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   static_cast<int>(f16x2_rows_ring_smem(4 * 256 * F16ROWS_MAXV))));
     c.ring_attr_set = true;
   }
-  const int64_t rows = bt.n * R;
-  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
-    constexpr bool HAS_OP = decltype(has_op)::value, BATCHED = decltype(batched)::value;
-    if (Cc <= 4 * 32 * F16ROWS_MAXV)
-      f16x2_rows_fused_kernel<32, HAS_OP, BATCHED><<<grid_for(c, (rows + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b,
-                                                                                             words, k, bt);
+  const int64_t rows = concat ? R : bt.n * R, row_len = concat ? bt.n * Cc : Cc;
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched, auto cat) {
+    constexpr bool HAS_OP = decltype(has_op)::value, BATCHED = decltype(batched)::value, CONCAT = decltype(cat)::value;
+    if (row_len <= 4 * 32 * F16ROWS_MAXV)
+      f16x2_rows_fused_kernel<32, HAS_OP, BATCHED, CONCAT><<<grid_for(c, (rows + 7) / 8, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb,
+                                                                                                     ld_b, words, k, bt);
     else if (ring)
       f16x2_rows_ring_kernel<<<grid_for(c, R, 2), 256, f16x2_rows_ring_smem(Cc), s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words);
     else
-      f16x2_rows_fused_kernel<256, HAS_OP, BATCHED><<<grid_for(c, rows, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b, words, k,
-                                                                                        bt);
-  });
+      f16x2_rows_fused_kernel<256, HAS_OP, BATCHED, CONCAT><<<grid_for(c, rows, 4), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b,
+                                                                                                words, k, bt);
+  }, concat);
 }
 
 // F16X3, one scale per column of fp32 rows [R][Cc]: the abs-max word of every column (zeroed here, then strip reductions
-// combined by atomicMax).  A column's scale needs the whole column, so the split is a second pass.
+// combined by atomicMax).  A column's scale needs the whole column, so the split is a second pass.  concat: one word per
+// column over every problem of the batch.
 int f16x2_col_scales(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint32_t *words, cudaStream_t s,
-                     const OperandOp *op = nullptr, const Batch &bt = Batch()) {
-  CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(bt.n * Cc) * sizeof(uint32_t), s));
+                     const OperandOp *op = nullptr, const Batch &bt = Batch(), bool concat = false) {
+  CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>((concat ? 1 : bt.n) * Cc) * sizeof(uint32_t), s));
   const int64_t items = ((Cc + 3) / 4) * ((R + ABSMAX_COL_ROWS - 1) / ABSMAX_COL_ROWS) * bt.n;
-  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
-    absmax_mn_kernel<true, decltype(has_op)::value, decltype(batched)::value><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(
-        src, R, Cc, src_ld, words, k, bt);
-  });
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched, auto cat) {
+    constexpr bool HAS_OP = decltype(has_op)::value, BATCHED = decltype(batched)::value, CONCAT = decltype(cat)::value;
+    absmax_mn_kernel<true, HAS_OP, BATCHED, CONCAT><<<grid_for(c, (items + 255) / 256, 8), 256, 0, s>>>(src, R, Cc, src_ld, words, k,
+                                                                                                       bt);
+  }, concat);
 }
 // F16X3, one scale per column: the two fp16 pieces [R][ld_b] of fp32 rows [R][Cc] against the columns' scale words
 int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *hb, uint16_t *lb, int64_t ld_b,
-                    const uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr, const Batch &bt = Batch()) {
+                    const uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr, const Batch &bt = Batch(),
+                    bool concat = false) {
   const int64_t items = ((Cc + 255) / 256) * ((R + SPLIT_ROWS - 1) / SPLIT_ROWS) * bt.n;
-  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched) {
-    split_rows_f16x2_kernel<true, decltype(has_op)::value, decltype(batched)::value><<<grid_for(c, items, 8), 256, 0, s>>>(
-        src, R, Cc, src_ld, hb, lb, ld_b, words, k, bt);
-  });
+  return launch_prep(op, bt, [&](auto has_op, const OperandOp &k, auto batched, auto cat) {
+    constexpr bool HAS_OP = decltype(has_op)::value, BATCHED = decltype(batched)::value, CONCAT = decltype(cat)::value;
+    split_rows_f16x2_kernel<true, HAS_OP, BATCHED, CONCAT><<<grid_for(c, items, 8), 256, 0, s>>>(src, R, Cc, src_ld, hb, lb, ld_b,
+                                                                                                words, k, bt);
+  }, concat);
 }
 
 // An im2col source (Operand::conv): every image's windows as K-major rows [batch][mn][ld] (split.cuh: im2col_rows_kernel) in
@@ -596,23 +608,31 @@ int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst
 // A batched operand (o.batch > 0) is prepared in the same launches, every problem's pieces and scale words stacked; its
 // maps are rank 3.  It is read in place only where every problem is: TMA needs a positive batch stride of whole 16-byte
 // units, the preparation kernels 16-byte aligned rows (operand and aux) in every problem.
+// A concatenated batch (o.concat) takes the same rows with the CONCAT kernels -- K-major: each row is the problems' rows laid
+// end to end; MN-major (F16X3): the problems' rows stacked, one scale word per column -- into workspace read through rank-2
+// maps of extent batch * k.  It is never read in place: one 2-D map cannot address the problems' segments.
 template <int ESZ>
 int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w, int block_mn,
                     OperandMaps *m, bool *used_ws, cudaStream_t s, const OperandOp *op = nullptr) {
   const bool conv = o.conv != nullptr;   // (fp32, no op)
   const Major mj = conv ? K_MAJOR : classify(o, ESZ);
   const Batch bt = batch_of(o);
+  const bool cat = o.concat;
+  const int64_t kk = cat ? bt.n * o.k : o.k;                 // k extent of the operand the tensor-core kernel reads
   const bool rows_ok = bt.n == 1 || ((o.s_b * ESZ) % 16 == 0 && (!op || !op->aux || o.aux_sb % 4 == 0));
   const bool map_ok = bt.n == 1 || (o.s_b > 0 && o.s_b < (static_cast<int64_t>(1) << 40) / ESZ);
   const bool tma_layout = (mj == K_MAJOR || (mj == MN_MAJOR && (ESZ == 2 || mode == SPLIT_F16X2))) && rows_ok;
-  const bool in_place = !conv && tma_layout && (mode == SPLIT_NONE ? !op && map_ok : !op || op_same_layout(o, *op));
+  const bool in_place = !conv && tma_layout && (mode == SPLIT_NONE ? !op && map_ok && !cat : !op || op_same_layout(o, *op));
   const Major out_mj = in_place ? mj : K_MAJOR;              // layout of the arrays the tensor-core kernel reads
-  const int64_t R = (out_mj == K_MAJOR) ? o.mn : o.k;        // their rows
-  const int64_t Cc = (out_mj == K_MAJOR) ? o.k : o.mn;       // their contiguous extent
+  const int64_t R = (out_mj == K_MAJOR) ? o.mn : o.k;        // their rows (per problem)
+  const int64_t Cc = (out_mj == K_MAJOR) ? o.k : o.mn;       // their contiguous extent (per problem)
   const int64_t src_ld = (mj == K_MAJOR) ? o.s_mn : o.s_k;   // row pitch of the operand, read in place
-  const int64_t ld = round_up(Cc, 16 / ESZ);
+  // the prepared arrays: rows_p rows of row_len elements (a concatenated K-major operand: the problems' rows end to end)
+  const bool cat_rows = cat && out_mj == K_MAJOR;
+  const int64_t rows_p = cat_rows ? R : bt.n * R, row_len = cat_rows ? bt.n * Cc : Cc;
+  const int64_t ld = round_up(row_len, 16 / ESZ);
   // rank-3 maps of a batched launch: `depth` matrices (1: shared by the batch) `d_stride(pitch)` elements apart
-  const int64_t depth = o.batch > 0 ? bt.n : 0;
+  const int64_t depth = o.batch > 0 && !cat ? bt.n : 0;
   auto d_stride = [&](int64_t pitch) { return bt.n > 1 ? (in_place && mode == SPLIT_NONE ? o.s_b : R * pitch) : R * pitch; };
   m->mn_major = (out_mj == MN_MAJOR);
   int rc;
@@ -629,44 +649,44 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
     const OperandOp kop = op ? kernel_op(*op, out_mj == MN_MAJOR) : OperandOp();
     const OperandOp *on_load = (in_place && op) ? &kop : nullptr;
     if (mode == SPLIT_F16X2) {
-      const int64_t ld_b = round_up(Cc, 8);
-      const size_t bytes_b = static_cast<size_t>(bt.n * R) * ld_b * 2;
+      const int64_t ld_b = round_up(row_len, 8);
+      const size_t bytes_b = static_cast<size_t>(rows_p) * ld_b * 2;
       if ((rc = ensure(*w.p0, bytes_b))) return rc;
       if ((rc = ensure(*w.p1, bytes_b))) return rc;
-      if (c.f16s.bytes < static_cast<size_t>(w.amax_off + bt.n * o.mn) * sizeof(uint32_t))
+      if (c.f16s.bytes < static_cast<size_t>(w.amax_off + (cat ? 1 : bt.n) * o.mn) * sizeof(uint32_t))
         return set_error(LASER_B200_ECUDA, "internal: F16X3 scale buffer not sized for this operand");
       uint16_t *hb = static_cast<uint16_t *>(w.p0->ptr), *lb = static_cast<uint16_t *>(w.p1->ptr);
       uint32_t *words = static_cast<uint32_t *>(c.f16s.ptr) + w.amax_off;
       if (conv) {
         rc = im2col_rows(c, o, mode, nullptr, nullptr, hb, lb, ld_b, words, s);
-      } else if (!in_place) {   // the gathered problems are stacked rows: one plain row pass over all of them
+      } else if (!in_place) {   // the gathered problems are stacked (concatenated) rows: one plain row pass over all of them
         if ((rc = gather<float>(c, o, *w.gather, nullptr, s, op))) return rc;
-        rc = f16x2_rows(c, static_cast<const float *>(w.gather->ptr), bt.n * R, Cc, ld, hb, lb, ld_b, words, s);
+        rc = f16x2_rows(c, static_cast<const float *>(w.gather->ptr), rows_p, row_len, ld, hb, lb, ld_b, words, s);
       } else if (out_mj == K_MAJOR) {
-        rc = f16x2_rows(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load, bt);
+        rc = f16x2_rows(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load, bt, cat);
       } else {
-        if ((rc = f16x2_col_scales(c, src, R, Cc, src_ld, words, s, on_load, bt))) return rc;
-        rc = f16x2_col_split(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load, bt);
+        if ((rc = f16x2_col_scales(c, src, R, Cc, src_ld, words, s, on_load, bt, cat))) return rc;
+        rc = f16x2_col_split(c, src, R, Cc, src_ld, hb, lb, ld_b, words, s, on_load, bt, cat);
       }
       if (rc) return rc;
-      if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, o.k, ld_b, block_mn, depth, d_stride(ld_b)))) return rc;
-      return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, o.k, ld_b, block_mn, depth, d_stride(ld_b));
+      if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, kk, ld_b, block_mn, depth, d_stride(ld_b)))) return rc;
+      return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, kk, ld_b, block_mn, depth, d_stride(ld_b));
     }
     if (!in_place && !conv) {
       rc = (mode == SPLIT_TF32) ? gather<float, 1>(c, o, *w.p0, w.p1, s, op) : gather<float>(c, o, *w.p0, nullptr, s, op);
     } else {   // TF32X3 K-major, or an im2col source (TF32X3, TF32X1)
-      const size_t bytes = static_cast<size_t>(bt.n * R) * ld * sizeof(float);
+      const size_t bytes = static_cast<size_t>(rows_p) * ld * sizeof(float);
       if ((rc = ensure(*w.p0, bytes))) return rc;
       if (mode == SPLIT_TF32 && (rc = ensure(*w.p1, bytes))) return rc;
       float *p0 = static_cast<float *>(w.p0->ptr), *p1 = mode == SPLIT_TF32 ? static_cast<float *>(w.p1->ptr) : nullptr;
       rc = conv ? im2col_rows(c, o, mode, p0, p1, nullptr, nullptr, ld, nullptr, s)
-                : tf32_split(c, src, R, Cc, src_ld, p0, p1, ld, s, on_load, bt);
+                : tf32_split(c, src, R, Cc, src_ld, p0, p1, ld, s, on_load, bt, cat);
     }
     if (rc) return rc;
   }
-  if ((rc = operand_map(c, &m->p0, ESZ, w.p0->ptr, out_mj, o.mn, o.k, ld, block_mn, depth, d_stride(ld)))) return rc;
+  if ((rc = operand_map(c, &m->p0, ESZ, w.p0->ptr, out_mj, o.mn, kk, ld, block_mn, depth, d_stride(ld)))) return rc;
   m->p1 = m->p0;
-  if (mode == SPLIT_TF32) return operand_map(c, &m->p1, ESZ, w.p1->ptr, out_mj, o.mn, o.k, ld, block_mn, depth, d_stride(ld));
+  if (mode == SPLIT_TF32) return operand_map(c, &m->p1, ESZ, w.p1->ptr, out_mj, o.mn, kk, ld, block_mn, depth, d_stride(ld));
   return LASER_B200_OK;
 }
 
@@ -688,10 +708,12 @@ inline TcKind tc_kind_of_path(int path) {
 }
 inline SplitMode split_mode(TcKind k) { return k == TC_TF32X3 ? SPLIT_TF32 : k == TC_F16X3 ? SPLIT_F16X2 : SPLIT_NONE; }
 
-// a batched call: `batch` problems, operand X of problem b at X + b * X_stride (0: the batch shares it)
+// a batched call: `batch` problems, operand X of problem b at X + b * X_stride (0: the batch shares it).  concat: the sum of
+// the problems' products into one C (C unused), i.e. one product over the operands concatenated along k (Operand::concat).
 struct BatchArgs {
   int64_t batch;
   int64_t A, B, C, auxA, auxB;
+  bool concat = false;
 };
 
 // launch the tensor-core kernel on prepared operands (c.mu held by the caller).  bat: a batched launch (tc_params.h; the maps
@@ -784,18 +806,23 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   // stream); everything that does not read B -- the preparation of A -- is queued before the wait.
   // opA / opB: operand ops applied while the operands are prepared (fp32 only)
   // convB: B is an im2col source, the images at B (batched: bat->B floats apart; rsB, csB unused)
-  if (M > 0x7fffffffLL || N > 0x7fffffffLL || K > 0x7fffffffLL)
+  // bat->concat: one product of extent batch * K over the concatenated operands (one problem for the GEMM: rank-2 maps, one
+  // scale word per row of A and column of B)
+  const bool cat = bat && bat->concat;
+  const int64_t Kt = cat ? bat->batch * K : K;   // (the entry bounds batch * K by INT64_MAX)
+  if (M > 0x7fffffffLL || N > 0x7fffffffLL || Kt > 0x7fffffffLL)
     return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: extents must fit in int32");
   std::lock_guard<std::mutex> lk(c.mu);  // workspace + descriptor construction are per context
   const SplitMode mode = split_mode(kind);
   Operand oa{A, M, K, rsA, csA};
   Operand ob{B, N, K, csB, rsB};
-  // bat: every problem's operand in the same launches (an operand -- op included -- that the batch shares: prepared once)
-  const bool a_shared = bat && bat->A == 0 && (!opA || !opA->aux || bat->auxA == 0);
-  const bool b_shared = bat && bat->B == 0 && (!opB || !opB->aux || bat->auxB == 0);
+  // bat: every problem's operand in the same launches (an operand -- op included -- that the batch shares: prepared once;
+  // concatenated: once per segment)
+  const bool a_shared = bat && !cat && bat->A == 0 && (!opA || !opA->aux || bat->auxA == 0);
+  const bool b_shared = bat && !cat && bat->B == 0 && (!opB || !opB->aux || bat->auxB == 0);
   if (bat) {
-    oa.batch = a_shared ? 1 : bat->batch; oa.s_b = bat->A; oa.aux_sb = bat->auxA;
-    ob.batch = b_shared ? 1 : bat->batch; ob.s_b = bat->B; ob.aux_sb = bat->auxB;
+    oa.batch = a_shared ? 1 : bat->batch; oa.s_b = bat->A; oa.aux_sb = bat->auxA; oa.concat = cat;
+    ob.batch = b_shared ? 1 : bat->batch; ob.s_b = bat->B; ob.aux_sb = bat->auxB; ob.concat = cat;
   }
   ob.conv = convB;
   OperandMaps ma, mb;
@@ -807,7 +834,7 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   if (rc) return rc;
   int64_t f16_b_off = 0;
   if (mode == SPLIT_F16X2 &&
-      (rc = f16_scales(c, batch_of(oa).n * M, batch_of(ob).n * N, &f16_b_off)))
+      (rc = f16_scales(c, (cat ? 1 : batch_of(oa).n) * M, (cat ? 1 : batch_of(ob).n) * N, &f16_b_off)))
     return rc;
   if ((rc = prepare_operand<SRC_ESZ>(c, oa, mode, ws_of_A(c), TC_BLOCK_M, &ma, &used_ws, s, opA))) return rc;
   if (b_ready) CUDA_TRY(cudaStreamWaitEvent(s, b_ready, 0));
@@ -816,8 +843,8 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   if ((rc = prep.close())) return rc;
   const F16Scales f16{static_cast<const uint32_t *>(c.f16s.ptr), static_cast<const uint32_t *>(c.f16s.ptr) + f16_b_off};
   // (with profiling on, an event record sits between the last preparation kernel and the GEMM: no dependent launch then)
-  rc = tc_run<OutT>(c, kind, M, N, K, alpha, ma, mb, beta, C, rsC, csC, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
-                    prep_launches > 0 && !c.profiling, bat, a_shared, b_shared);
+  rc = tc_run<OutT>(c, kind, M, N, Kt, alpha, ma, mb, beta, C, rsC, csC, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
+                    prep_launches > 0 && !c.profiling, cat ? nullptr : bat, a_shared, b_shared);
   if (rc) return rc;
   if (used_ws) CUDA_TRY(cudaEventRecord(c.ws_free, s));
   return LASER_B200_OK;
@@ -1220,6 +1247,62 @@ int batched_fused_entry(int64_t batch, int64_t M, int64_t N, int64_t K, float al
 }
 
 // ---------------------------------------------------------------------------------------
+//   batch-reduced fused product: the sum of a batch's products, one product over the operands concatenated along k
+// ---------------------------------------------------------------------------------------
+// Exact path: the gather writes each operand concatenated (op applied) into compact [mn][batch * K] rows, and the unchanged
+// exact kernel multiplies those, so the path stays bit-identical to the CPU reference over the concatenation.
+int batch_reduce_simt(Ctx &c, const BatchArgs &bat, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA,
+                      int64_t csA, const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
+                      cudaStream_t s, const Epilogue &epi, const OperandOp *opA, const OperandOp *opB) {
+  const int64_t Kt = bat.batch * K, ld = round_up(Kt, 4);
+  Operand oa{A, M, K, rsA, csA, bat.batch, bat.A, bat.auxA}, ob{B, N, K, csB, rsB, bat.batch, bat.B, bat.auxB};
+  oa.concat = ob.concat = true;
+  std::lock_guard<std::mutex> lk(c.mu);   // the gather buffers are workspace
+  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
+  int rc;
+  if ((rc = gather<float>(c, oa, c.gather[0], nullptr, s, opA))) return rc;
+  if ((rc = gather<float>(c, ob, c.gather[1], nullptr, s, opB))) return rc;
+  if ((rc = gemm_simt<float>(c, M, N, Kt, alpha, static_cast<const float *>(c.gather[0].ptr), ld, 1,
+                             static_cast<const float *>(c.gather[1].ptr), 1, ld, beta, C, rsC, csC, s, epi)))
+    return rc;
+  CUDA_TRY(cudaEventRecord(c.ws_free, s));
+  return LASER_B200_OK;
+}
+
+// laser_b200_gemm_strided_batch_reduce_f32_fused_dev: C <- act(alpha * sum_b opA(A_b) * opB(B_b) + beta * C + bias), the fused
+// call over A^ = [opA(A_0) | .. | opA(A_{n-1})] (M x nK) and B^ = [opB(B_0); ..; opB(B_{n-1})] (nK x N).  One chunk always:
+// chunking a sum would round C between chunks and apply the activation too early.
+int batch_reduce_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
+                     const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
+                     const laser_b200_batch_strides *bs, const OperandOp *opA, const OperandOp *opB, const Epilogue &epi, int path,
+                     void *stream) {
+  if (batch < 0) return set_error(LASER_B200_EINVAL, "negative batch %lld", (long long)batch);
+  if (batch > 0 && !bs) return set_error(LASER_B200_EINVAL, "batchStrides is NULL");
+  if (batch > 0 && bs->C != 0)
+    return set_error(LASER_B200_EINVAL, "batchStrides->C is %lld: the batch sums into one C", (long long)bs->C);
+  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
+    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  int rc = check_args(M, N, K, A, B, C);
+  if (rc == -1 || batch == 0) return LASER_B200_OK;
+  if (rc) return rc;
+  if (batch == 1) return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, epi, nullptr, opA, opB);
+  if (K > INT64_MAX / batch) return set_error(LASER_B200_EUNSUPPORTED, "batch * K overflows int64");
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, batch * K, epi, /*operand_op=*/true);
+  const BatchArgs bat{batch, bs->A, bs->B, 0, bs->auxA, bs->auxB, true};
+  if (path == LASER_B200_PATH_SIMT)
+    rc = batch_reduce_simt(*c, bat, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, opA, opB);
+  else
+    rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, nullptr,
+                           opA, opB, &bat);
+  if (rc) return rc;
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
+}
+
+// ---------------------------------------------------------------------------------------
 //     fused convolution: im2col folded into the preparation of B, the images of a chunk in one GEMM launch
 // ---------------------------------------------------------------------------------------
 // Exact path, `images` images: their windows as plain K-major rows in the gather workspace, one batched exact-kernel launch
@@ -1592,6 +1675,20 @@ int laser_b200_gemm_strided_f32_fused_dev(int64_t M, int64_t N, int64_t K, float
   if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
   if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
   return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, e, nullptr, pa, pb);
+}
+int laser_b200_gemm_strided_batch_reduce_f32_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A,
+                                                       int64_t rsA, int64_t csA, const float *B, int64_t rsB, int64_t csB, float beta,
+                                                       float *C, int64_t rsC, int64_t csC, const laser_b200_batch_strides *batchStrides,
+                                                       const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
+                                                       const laser_b200_epilogue *epi, int path, void *stream) {
+  Epilogue e;
+  OperandOp oa, ob;
+  const OperandOp *pa, *pb;
+  int rc;
+  if ((rc = epilogue_of(epi, &e))) return rc;
+  if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
+  if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
+  return batch_reduce_dev(batch, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, batchStrides, pa, pb, e, path, stream);
 }
 int laser_b200_gemm_strided_f64_dev(int64_t M, int64_t N, int64_t K, double alpha, const double *A,
                                     int64_t rsA, int64_t csA, const double *B, int64_t rsB,

@@ -118,35 +118,80 @@ __device__ __forceinline__ int64_t batch_row(int64_t g, int64_t R, const Batch &
   }
 }
 
+// ---- batch-reduced preparation: the problems concatenated along k ----------------------------------------------------
+// The kernels below also take `template <bool CONCAT>` (only with BATCHED; false: the kernels above and their batched
+// twins).  A CONCAT kernel prepares ONE operand of extent bt.n * k, whose b-th k-segment is problem b's operand: the operand
+// of a sum of products over the batch.  A kernel whose rows run along mn (K-major) writes row r as the problems' rows r laid
+// end to end, [R][bt.n * Cc]; one whose rows run along k (MN-major) writes the problems' rows stacked as BATCHED does,
+// [bt.n * R][Cc], with ONE scale word per column for all of them.
+// Elements c .. c+3 of row r of the rows laid end to end (0 past bt.n * Cc), op applied: one vector load where the four lie
+// in one problem at a 16-byte boundary (the host passes 16-byte aligned rows, aux rows and problem offsets), element by
+// element across a boundary.  int32 positions: the tensor-core path bounds bt.n * Cc by 2^31.
+template <bool HAS_OP>
+__device__ __forceinline__ float4 concat_vec(const float *src, int64_t src_ld, const OperandOp &op, const Batch &bt, int64_t r,
+                                             int64_t c, int64_t Cc) {
+  const int seg = static_cast<int>(Cc);
+  int b = static_cast<int>(c) / seg;
+  int k = static_cast<int>(c) - b * seg;
+  if ((k & 3) == 0 && k + 4 <= seg) {
+    float4 v = *reinterpret_cast<const float4 *>(src + b * bt.bs + r * src_ld + k);
+    if constexpr (HAS_OP) {
+      float4 y = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      if (op.aux) y = *reinterpret_cast<const float4 *>(op.aux + b * bt.aux_bs + r * op.aux_sr + k);
+      v.x = operand_op(op.op, v.x, y.x); v.y = operand_op(op.op, v.y, y.y);
+      v.z = operand_op(op.op, v.z, y.z); v.w = operand_op(op.op, v.w, y.w);
+    }
+    return v;
+  }
+  float e[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    while (k >= seg) { k -= seg; ++b; }   // (segments shorter than 4 floats: more than one boundary)
+    float x = 0.0f;
+    if (b < bt.n) {
+      x = src[b * bt.bs + r * src_ld + k];
+      if constexpr (HAS_OP) x = operand_op(op.op, x, op.aux ? op.aux[b * bt.aux_bs + r * op.aux_sr + k] : 0.0f);
+    }
+    e[i] = x;
+    ++k;
+  }
+  return make_float4(e[0], e[1], e[2], e[3]);
+}
+
 // src: R rows of Cc contiguous floats, leading dimension src_ld (16-byte aligned rows).
 // hi/lo: compact, leading dimension dst_ld (multiple of 4).
-template <bool HAS_OP = false, bool BATCHED = false>
+template <bool HAS_OP = false, bool BATCHED = false, bool CONCAT = false>
 __global__ void __launch_bounds__(256)
 split_rows_tf32_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld,
                        float *__restrict__ hi, float *__restrict__ lo, int64_t dst_ld, OperandOp op = OperandOp(),
                        Batch bt = Batch()) {
+  static_assert(!CONCAT || BATCHED, "a concatenation is of a batch");
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
-  const int64_t vec_per_row = (Cc + 3) >> 2;
-  const int64_t total = (BATCHED ? bt.n * R : R) * vec_per_row;
+  const int64_t vec_per_row = ((CONCAT ? bt.n * Cc : Cc) + 3) >> 2;
+  const int64_t total = (BATCHED && !CONCAT ? bt.n * R : R) * vec_per_row;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int64_t r = i / vec_per_row;
     const int64_t c = (i - r * vec_per_row) << 2;
-    const float *sp = src;
-    OperandOp o = op;
-    const int64_t rl = batch_row<BATCHED>(r, R, bt, sp, o);
-    const float *s = sp + rl * src_ld + c;
     float4 v;
-    if (c + 4 <= Cc) {
-      v = *reinterpret_cast<const float4 *>(s);
+    if constexpr (CONCAT) {
+      v = concat_vec<HAS_OP>(src, src_ld, op, bt, r, c, Cc);
     } else {
-      v.x = s[0];
-      v.y = (c + 1 < Cc) ? s[1] : 0.0f;
-      v.z = (c + 2 < Cc) ? s[2] : 0.0f;
-      v.w = 0.0f;
+      const float *sp = src;
+      OperandOp o = op;
+      const int64_t rl = batch_row<BATCHED>(r, R, bt, sp, o);
+      const float *s = sp + rl * src_ld + c;
+      if (c + 4 <= Cc) {
+        v = *reinterpret_cast<const float4 *>(s);
+      } else {
+        v.x = s[0];
+        v.y = (c + 1 < Cc) ? s[1] : 0.0f;
+        v.z = (c + 2 < Cc) ? s[2] : 0.0f;
+        v.w = 0.0f;
+      }
+      if constexpr (HAS_OP && BATCHED) v = op_vec(o, v, rl, c, Cc);
+      else if constexpr (HAS_OP) v = op_vec(op, v, r, c, Cc);
     }
-    if constexpr (HAS_OP && BATCHED) v = op_vec(o, v, rl, c, Cc);
-    else if constexpr (HAS_OP) v = op_vec(op, v, r, c, Cc);
     float4 h, l;
     h.x = tf32_rna(v.x); l.x = tf32_lo(v.x, h.x);
     h.y = tf32_rna(v.y); l.y = tf32_lo(v.y, h.y);
@@ -169,12 +214,13 @@ __device__ __forceinline__ uint32_t finite_abs_bits(float f) {
 }
 constexpr int ABSMAX_ROW_CHUNK = 1024;   // floats of one row reduced by one warp pass (32 lanes x 8 x float4)
 constexpr int ABSMAX_COL_ROWS = 64;      // rows of a 4-column strip reduced by one thread
-template <bool PER_COL, bool HAS_OP = false, bool BATCHED = false>
+template <bool PER_COL, bool HAS_OP = false, bool BATCHED = false, bool CONCAT = false>
 __global__ void __launch_bounds__(256)
 absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld, uint32_t *__restrict__ out,
                  OperandOp op = OperandOp(), Batch bt = Batch()) {
   static_assert(PER_COL || !HAS_OP, "a K-major operand with an op takes the fused row kernel");
   static_assert(PER_COL || !BATCHED, "a K-major operand takes the fused row kernel");
+  static_assert(!CONCAT || BATCHED, "a concatenation is of a batch");
   if constexpr (!PER_COL) {
     // warp w takes (row, chunk) items; lanes read float4s 128 floats apart; butterfly max; one atomic per item
     const int lane = threadIdx.x & 31;
@@ -220,7 +266,7 @@ absmax_mn_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t s
         const int64_t b = rb / rblocks;
         rb -= b * rblocks;
         batch_row<true>(b * R, R, bt, src_b, o);
-        out_b += b * Cc;
+        if constexpr (!CONCAT) out_b += b * Cc;   // (CONCAT: one word per column over every problem)
       }
       const int64_t r1 = (rb + 1) * ABSMAX_COL_ROWS < R ? (rb + 1) * ABSMAX_COL_ROWS : R;
       uint32_t m0 = 0u, m1 = 0u, m2 = 0u, m3 = 0u;
@@ -265,26 +311,27 @@ __device__ __forceinline__ void store_f16x2_vec(float4 v, float s, uint16_t *hro
 // thread; what is left of a longer row is read twice, the second time from L2), reduces the abs-max, writes the word and
 // both fp16 pieces: 4 bytes read + 4 written per element, against 8 + 4 for abs-max and split as two kernels.
 constexpr int F16ROWS_MAXV = 8;
-template <int GROUP, bool HAS_OP = false, bool BATCHED = false>
+template <int GROUP, bool HAS_OP = false, bool BATCHED = false, bool CONCAT = false>
 __global__ void __launch_bounds__(256, 4)
 f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld, uint16_t *__restrict__ hb,
                         uint16_t *__restrict__ lb, int64_t ld_b, uint32_t *__restrict__ absmax, OperandOp op = OperandOp(),
                         Batch bt = Batch()) {
   static_assert(GROUP == 32 || GROUP == 256, "a warp or the CTA per row");
+  static_assert(!CONCAT || BATCHED, "a concatenation is of a batch");
   __shared__ uint32_t red[2][8];
   ptx::griddep_launch_dependents();
   const int tid = static_cast<int>(threadIdx.x) % GROUP;
   const int64_t per_cta = 256 / GROUP;
   const int64_t first = static_cast<int64_t>(blockIdx.x) * per_cta + static_cast<int64_t>(threadIdx.x) / GROUP;
   const int64_t step = static_cast<int64_t>(gridDim.x) * per_cta;
-  const int64_t nvec = (Cc + 3) >> 2;
+  const int64_t nvec = ((CONCAT ? bt.n * Cc : Cc) + 3) >> 2;
   int parity = 0;
   // GROUP == 256: every thread of the CTA runs the same number of iterations (the loop holds a __syncthreads)
-  const int64_t rows = BATCHED ? bt.n * R : R;
+  const int64_t rows = BATCHED && !CONCAT ? bt.n * R : R;
   for (int64_t r = first; r < rows; r += step) {
     const float *sp = src;
     OperandOp o = op;
-    const int64_t rl = batch_row<BATCHED>(r, R, bt, sp, o);
+    const int64_t rl = batch_row<BATCHED && !CONCAT>(r, R, bt, sp, o);
     const float *row = sp + rl * src_ld;
     float4 v[F16ROWS_MAXV];
     uint32_t m = 0u;
@@ -292,14 +339,23 @@ f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
     for (int i = 0; i < F16ROWS_MAXV; ++i) {
       const int64_t idx = tid + static_cast<int64_t>(i) * GROUP;
       if (idx < nvec) {
-        v[i] = load_row_vec(row, idx << 2, Cc);
-        if constexpr (HAS_OP) v[i] = op_vec(o, v[i], rl, idx << 2, Cc);
+        if constexpr (CONCAT) {
+          v[i] = concat_vec<HAS_OP>(src, src_ld, op, bt, r, idx << 2, Cc);
+        } else {
+          v[i] = load_row_vec(row, idx << 2, Cc);
+          if constexpr (HAS_OP) v[i] = op_vec(o, v[i], rl, idx << 2, Cc);
+        }
         m = max(max(m, finite_abs_bits(v[i].x)), max(finite_abs_bits(v[i].y), max(finite_abs_bits(v[i].z), finite_abs_bits(v[i].w))));
       }
     }
     for (int64_t idx = tid + static_cast<int64_t>(F16ROWS_MAXV) * GROUP; idx < nvec; idx += GROUP) {
-      float4 t = load_row_vec(row, idx << 2, Cc);
-      if constexpr (HAS_OP) t = op_vec(o, t, rl, idx << 2, Cc);
+      float4 t;
+      if constexpr (CONCAT) {
+        t = concat_vec<HAS_OP>(src, src_ld, op, bt, r, idx << 2, Cc);
+      } else {
+        t = load_row_vec(row, idx << 2, Cc);
+        if constexpr (HAS_OP) t = op_vec(o, t, rl, idx << 2, Cc);
+      }
       m = max(max(m, finite_abs_bits(t.x)), max(finite_abs_bits(t.y), max(finite_abs_bits(t.z), finite_abs_bits(t.w))));
     }
     float mf = __uint_as_float(m);     // non-negative finite: fmaxf orders them like the integers
@@ -322,7 +378,8 @@ f16x2_rows_fused_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
       if (idx < nvec) store_f16x2_vec(v[i], s, hrow, lrow, idx << 2);
     }
     for (int64_t idx = tid + static_cast<int64_t>(F16ROWS_MAXV) * GROUP; idx < nvec; idx += GROUP) {
-      if constexpr (HAS_OP) store_f16x2_vec(op_vec(o, load_row_vec(row, idx << 2, Cc), rl, idx << 2, Cc), s, hrow, lrow, idx << 2);
+      if constexpr (CONCAT) store_f16x2_vec(concat_vec<HAS_OP>(src, src_ld, op, bt, r, idx << 2, Cc), s, hrow, lrow, idx << 2);
+      else if constexpr (HAS_OP) store_f16x2_vec(op_vec(o, load_row_vec(row, idx << 2, Cc), rl, idx << 2, Cc), s, hrow, lrow, idx << 2);
       else store_f16x2_vec(load_row_vec(row, idx << 2, Cc), s, hrow, lrow, idx << 2);
     }
   }
@@ -414,12 +471,13 @@ inline bool f16x2_rows_ring_ok(const float *src, int64_t Cc, int64_t src_ld) {
 // SPLIT_ROWS rows): a thread owns 4 columns of the strip -- for PER_COL their four scales are computed once -- and walks
 // the rows of the block, adjacent threads reading adjacent float4s.
 constexpr int SPLIT_ROWS = 64;
-template <bool PER_COL, bool HAS_OP = false, bool BATCHED = false>
+template <bool PER_COL, bool HAS_OP = false, bool BATCHED = false, bool CONCAT = false>
 __global__ void __launch_bounds__(256)
 split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, int64_t src_ld,
                         uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld_b,
                         const uint32_t *__restrict__ absmax, OperandOp op = OperandOp(), Batch bt = Batch()) {
   static_assert(PER_COL || !BATCHED, "a K-major operand takes the fused row kernel");
+  static_assert(!CONCAT || BATCHED, "a concatenation is of a batch");
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   const int tx = static_cast<int>(threadIdx.x) & 63, ty = static_cast<int>(threadIdx.x) >> 6;   // 64 float4 columns x 4 row lanes
   const int64_t strips = (Cc + 255) >> 8;
@@ -437,7 +495,7 @@ split_rows_f16x2_kernel(const float *__restrict__ src, int64_t R, int64_t Cc, in
       const int64_t b = rb / rblocks;
       rb -= b * rblocks;
       batch_row<true>(b * R, R, bt, src_b, o);
-      absmax_b += b * Cc;
+      if constexpr (!CONCAT) absmax_b += b * Cc;
       hb_b += b * R * ld_b;
       lb_b += b * R * ld_b;
     }
@@ -578,13 +636,15 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, fl
 // store (along c) are coalesced.  SPLIT: also write lo (fp32 only).
 // MODE 0: plain copy; 1: fp32 hi/lo pieces (dst, dst_lo).
 // HAS_OP (fp32): the op is applied to each element as it is gathered (aux read with its own strides).
-template <typename T, int MODE, bool HAS_OP = false, bool BATCHED = false>
+// CONCAT: problem b's [R][Cc] is written to columns b * Cc .. of the rows [R][ld] (ld >= bt.n * Cc).
+template <typename T, int MODE, bool HAS_OP = false, bool BATCHED = false, bool CONCAT = false>
 __global__ void __launch_bounds__(256)
 pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr, int64_t sc,
                     T *__restrict__ dst, T *__restrict__ dst_lo, int64_t ld, int read_along_r, OperandOp op = OperandOp(),
                     Batch bt = Batch()) {
   static_assert(!HAS_OP || sizeof(T) == 4, "operand ops are fp32 only");
   static_assert(!BATCHED || sizeof(T) == 4, "batched operands are fp32 only");
+  static_assert(!CONCAT || BATCHED, "a concatenation is of a batch");
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   __shared__ T tile[32][33];
   const int64_t tiles_c = (Cc + 31) >> 5;
@@ -601,8 +661,8 @@ pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr
       r0 -= (b * tiles_r) << 5;
       src_t += b * bt.bs;
       if (o.aux) o.aux += b * bt.aux_bs;
-      dst_t += b * R * ld;
-      if constexpr (MODE == 1) dlo_t += b * R * ld;
+      dst_t += CONCAT ? b * Cc : b * R * ld;   // (CONCAT: to columns b * Cc + c)
+      if constexpr (MODE == 1) dlo_t += CONCAT ? b * Cc : b * R * ld;
     }
     if (read_along_r) {
 #pragma unroll

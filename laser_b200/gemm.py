@@ -221,6 +221,24 @@ def gemm_strided_batched_fused(batch, M, N, K, alpha, A, rowStrideA, colStrideA,
         ctypes.byref(ob) if ob is not None else None, ctypes.byref(epi), path, stream))
 
 
+def gemm_strided_batch_reduce_fused(batch, M, N, K, alpha, A, rowStrideA, colStrideA, batchStrideA, B, rowStrideB, colStrideB,
+                                    batchStrideB, beta, C, rowStrideC, colStrideC, bias=None, bias_per_row=False,
+                                    activation="none", path=PATH_AUTO, stream=None, *, op_a=None, op_b=None):
+    """C <- act(alpha * sum_b opA(A_b) * opB(B_b) + beta*C + bias) on float32 DEVICE buffers (torch.addbmm): the sum of a
+    batch's products into one C, computed as one fused product over the operands concatenated along K.  A_b = A +
+    b * batchStrideA, B_b = B + b * batchStrideB; op_a / op_b as in gemm_strided_batched_fused, with the aux tensor's batch
+    stride last."""
+    pa, pb, pc, epi = _fused_args("gemm_strided_batch_reduce_fused", A, B, C, bias, bias_per_row, activation)
+    (oa, aux_a), (ob, aux_b) = _operand_op(op_a, batched=True), _operand_op(op_b, batched=True)
+    strides = _capi.BatchStrides(int(batchStrideA), int(batchStrideB), 0, aux_a, aux_b)
+    if stream is None:
+        stream = _current_stream()
+    check(lib().laser_b200_gemm_strided_batch_reduce_f32_fused_dev(
+        int(batch), M, N, K, float(alpha), pa, rowStrideA, colStrideA, pb, rowStrideB, colStrideB, float(beta), pc, rowStrideC,
+        colStrideC, ctypes.byref(strides), ctypes.byref(oa) if oa is not None else None,
+        ctypes.byref(ob) if ob is not None else None, ctypes.byref(epi), path, stream))
+
+
 def last_path():
     return lib().laser_b200_last_path()
 

@@ -121,6 +121,14 @@ proc laser_b200_gemm_strided_batched_f32_fused_dev*(batch, M, N, K: int64, alpha
     beta: float32, C: ptr float32, rowStrideC, colStrideC: int64,
     batchStrides: ptr LaserB200BatchStrides,
     opA, opB: ptr LaserB200OperandOp, epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
+# batch-reduced fused product (torch.addbmm): C <- act(alpha * sum_b opA(A_b) * opB(B_b) + beta * C + bias), one GEMM over
+# the operands concatenated along K; batchStrides.C must be 0
+proc laser_b200_gemm_strided_batch_reduce_f32_fused_dev*(batch, M, N, K: int64, alpha: float32,
+    A: ptr float32, rowStrideA, colStrideA: int64,
+    B: ptr float32, rowStrideB, colStrideB: int64,
+    beta: float32, C: ptr float32, rowStrideC, colStrideC: int64,
+    batchStrides: ptr LaserB200BatchStrides,
+    opA, opB: ptr LaserB200OperandOp, epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
 proc laser_b200_malloc*(devPtr: ptr pointer, bytes: csize_t): cint
 proc laser_b200_free*(devPtr: pointer): cint
 proc laser_b200_memcpy_h2d*(dst, src: pointer, bytes: csize_t): cint
