@@ -453,6 +453,32 @@ int laser_b200_conv2d_im2col_f32_dev(float *output, const float *input, const in
 int laser_b200_conv2d_f32_fused_dev(float *output, const float *input, const int64_t ishape[4],
                                     const float *kernel, const int64_t kshape[4], const int64_t padding[2],
                                     const int64_t strides[2], const laser_b200_epilogue *epi, int path, void *stream);
+/* Filter gradient of the fused convolution (derivatives applied while an operand is prepared for a backward product, and the
+ * im2col prepacker, of the reference's fusion roadmap, README.md:244-245 and :251; the reference has no backward convolution):
+ *   grad_kernel <- alpha * sum_n op(grad_output_n) * im2col(input_n)^T + beta * grad_kernel
+ * with input dense NCHW of shape ishape, grad_output dense NCHW [n][c_out][outH][outW] (conv2d_out_shape), and grad_kernel
+ * dense [c_out][c_in][kH][kW], i.e. [c_out][K] row-major with K = c_in * kH * kW in the im2col order of the forward call.
+ * op (NULL: none) is applied to grad_output -- e.g. LASER_B200_OP_RELU_GRAD with the forward call's output as aux, so the
+ * backward pass of a forward call with an activation is one call; the aux of a derivative op is a dense NCHW tensor of
+ * grad_output's shape (auxRowStride = outH * outW, auxColStride = 1; the images follow each other).  beta = 1 accumulates
+ * across micro-batches.  The call is the batch-reduced product over the images, its B operand prepared straight from the
+ * images (no im2col matrix, no workspace argument), and it runs as one chunk whatever LASER_B200_BATCH_WS_MB says: chunks
+ * would round grad_kernel between them.  grad_kernel is bit for bit what laser_b200_gemm_strided_batch_reduce_f32_fused_dev
+ * gives over materialised im2col matrices read transposed, on the same path.
+ *   Geometry checks of conv2d_im2col_f32_dev.  PATH_AUTO decides as the batch-reduced product with an operand op does for
+ *   M = c_out, N = K, K' = n * outH * outW, so it never takes the N <= 4 GEMV shortcut.  The one case where that differs from
+ *   the batch-reduced call is a single image without op, K <= 4 and c_out >= 1024: there the batch-reduced call's PATH_AUTO
+ *   takes the GEMV and this entry does not, and the two agree bit for bit only on an explicit path.
+ *   1 x 1 kernels with unit strides and no padding read the images in place.
+ *   n = 0: LASER_B200_OK, nothing launched, grad_kernel untouched.  n * outH * outW must fit in int32 on the tensor-core
+ *   paths (LASER_B200_EUNSUPPORTED otherwise).
+ *   LASER_B200_EINVAL, before anything is launched: an unknown path or op, a derivative op without aux or with other aux
+ *   strides, a NULL pointer. */
+int laser_b200_conv2d_filter_grad_f32_fused_dev(float *grad_kernel, const float *input, const int64_t ishape[4],
+                                                const float *grad_output, const int64_t kshape[4],
+                                                const int64_t padding[2], const int64_t strides[2],
+                                                float alpha, float beta, const laser_b200_operand_op *op,
+                                                int path, void *stream);
 /* host pointers, synchronous, library-owned workspace */
 int laser_b200_conv2d_im2col_f32(float *output, const float *input, const int64_t ishape[4],
                                  const float *kernel, const int64_t kshape[4], const int64_t padding[2],

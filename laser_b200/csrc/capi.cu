@@ -375,7 +375,8 @@ struct Operand {
   // batch 1 with a batched launch is an operand the problems share.  0: a single problem, rank-2 maps.
   int64_t batch = 0, s_b = 0, aux_sb = 0;
   // an im2col source: B of a convolution, [mn = outH * outW][k = C * kH * kW] per image, read from the `batch` NCHW images at
-  // ptr, s_b floats apart (s_mn, s_k unused)
+  // ptr, s_b floats apart (s_mn, s_k unused).  With `concat`: a concatenated im2col source, the B of a convolution's filter
+  // gradient, [mn = C * kH * kW][k = outH * outW] per image, the `batch` images' k-segments end to end
   const ConvGeom *conv = nullptr;
   // a concatenated batch: the operand of a sum of products, [mn][batch * k], whose k-segment b is problem b's [mn][k] (s_b
   // apart, 0: the same matrix in every segment); prepared into compact workspace and read through rank-2 maps
@@ -576,29 +577,41 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
 
 // An im2col source (Operand::conv): every image's windows as K-major rows [batch][mn][ld] (split.cuh: im2col_rows_kernel) in
 // the format of `mode` -- words and fp16 pieces into hb / lb / words (F16X2), tf32 hi / lo into dst / dst_lo (TF32), the
-// values into dst (NONE: TF32X1 and the exact path)
+// values into dst (NONE: TF32X1 and the exact path).  A concatenated one (with Operand::concat): the tap rows [mn][ld] of
+// every image end to end (split.cuh: im2col_tap_rows_kernel), F16X2 after an abs-max pass over the same tiles.
 int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst_lo, uint16_t *hb, uint16_t *lb, int64_t ld,
                 uint32_t *words, cudaStream_t s) {
   const Im2colSrc q = im2col_src(*o.conv);
   const int64_t images = batch_of(o).n, rows = images * o.mn;
+  const int64_t tiles = o.mn * ((ld + TAP_SEG - 1) / TAP_SEG);
   const float *in = static_cast<const float *>(o.ptr);
-  auto launch = [&](auto m) {
+  auto launch = [&](auto m, auto absmax) {
     constexpr int MODE = decltype(m)::value, PER_SM = MODE == IM2COL_F16X2 ? 3 : 4;   // the kernel's launch bounds
-    if (ld <= 4 * 32 * F16ROWS_MAXV)
+    if (o.concat)
+      im2col_tap_rows_kernel<MODE, decltype(absmax)::value><<<grid_for(c, tiles, 8), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb,
+                                                                                                 ld, words);
+    else if (ld <= 4 * 32 * F16ROWS_MAXV)
       im2col_rows_kernel<MODE, 32><<<grid_for(c, (rows + 7) / 8, PER_SM), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb, ld, words);
     else
       im2col_rows_kernel<MODE, 256><<<grid_for(c, rows, PER_SM), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb, ld, words);
+    COUNT_LAUNCH();
+    CHECK_LAUNCH();
+    return LASER_B200_OK;
   };
-  if (mode == SPLIT_F16X2) launch(std::integral_constant<int, IM2COL_F16X2>());
-  else if (mode == SPLIT_TF32) launch(std::integral_constant<int, IM2COL_TF32>());
-  else launch(std::integral_constant<int, IM2COL_F32>());
-  COUNT_LAUNCH();
-  CHECK_LAUNCH();
-  return LASER_B200_OK;
+  if (mode == SPLIT_F16X2 && o.concat) {   // one word per tap row over every image
+    CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(o.mn) * sizeof(uint32_t), s));
+    const int rc = launch(std::integral_constant<int, IM2COL_F16X2>(), std::true_type());
+    if (rc) return rc;
+  }
+  if (mode == SPLIT_F16X2) return launch(std::integral_constant<int, IM2COL_F16X2>(), std::false_type());
+  if (mode == SPLIT_TF32) return launch(std::integral_constant<int, IM2COL_TF32>(), std::false_type());
+  return launch(std::integral_constant<int, IM2COL_F32>(), std::false_type());
 }
 
 // One operand of a tensor-core call: first the plan, then its steps.
 //   An im2col source: one pass from the images into the prepared rows, K-major like a gathered operand.
+//   A concatenated im2col source: the tap rows of every image end to end, K-major [mn][batch * k] (F16X3: an abs-max pass
+//     over the images first, then the split pass).
 //   bf16 K- or MN-major; TF32X1 K-major without op: TMA reads the caller's memory, no workspace.
 //   TF32X3 K-major; F16X3 K- or MN-major -- without op, or with aux laid out like the operand: the split reads the caller's
 //     memory and applies the op on load (F16X3 MN-major: all column scales first, then the split).
@@ -1250,18 +1263,27 @@ int batched_fused_entry(int64_t batch, int64_t M, int64_t N, int64_t K, float al
 //   batch-reduced fused product: the sum of a batch's products, one product over the operands concatenated along k
 // ---------------------------------------------------------------------------------------
 // Exact path: the gather writes each operand concatenated (op applied) into compact [mn][batch * K] rows, and the unchanged
-// exact kernel multiplies those, so the path stays bit-identical to the CPU reference over the concatenation.
+// exact kernel multiplies those, so the path stays bit-identical to the CPU reference over the concatenation.  convB: B is a
+// concatenated im2col source (the images at B, bat.B floats apart), its plain tap rows written by im2col_rows.
 int batch_reduce_simt(Ctx &c, const BatchArgs &bat, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA,
                       int64_t csA, const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
-                      cudaStream_t s, const Epilogue &epi, const OperandOp *opA, const OperandOp *opB) {
+                      cudaStream_t s, const Epilogue &epi, const OperandOp *opA, const OperandOp *opB,
+                      const ConvGeom *convB = nullptr) {
   const int64_t Kt = bat.batch * K, ld = round_up(Kt, 4);
   Operand oa{A, M, K, rsA, csA, bat.batch, bat.A, bat.auxA}, ob{B, N, K, csB, rsB, bat.batch, bat.B, bat.auxB};
   oa.concat = ob.concat = true;
+  ob.conv = convB;
   std::lock_guard<std::mutex> lk(c.mu);   // the gather buffers are workspace
   CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
   int rc;
   if ((rc = gather<float>(c, oa, c.gather[0], nullptr, s, opA))) return rc;
-  if ((rc = gather<float>(c, ob, c.gather[1], nullptr, s, opB))) return rc;
+  if (convB) {
+    if ((rc = ensure(c.gather[1], static_cast<size_t>(N) * ld * sizeof(float)))) return rc;
+    rc = im2col_rows(c, ob, SPLIT_NONE, static_cast<float *>(c.gather[1].ptr), nullptr, nullptr, nullptr, ld, nullptr, s);
+  } else {
+    rc = gather<float>(c, ob, c.gather[1], nullptr, s, opB);
+  }
+  if (rc) return rc;
   if ((rc = gemm_simt<float>(c, M, N, Kt, alpha, static_cast<const float *>(c.gather[0].ptr), ld, 1,
                              static_cast<const float *>(c.gather[1].ptr), 1, ld, beta, C, rsC, csC, s, epi)))
     return rc;
@@ -1366,6 +1388,52 @@ int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const
     }
     if (rc) return rc;
   }
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
+}
+
+// ---------------------------------------------------------------------------------------
+//   convolution filter gradient: one batch-reduced product whose B is prepared straight from the images
+// ---------------------------------------------------------------------------------------
+// laser_b200_conv2d_filter_grad_f32_fused_dev (capi_layers.inc checks the geometry):
+//   grad_kernel <- alpha * sum_n op(grad_output_n) * im2col(input_n)^T + beta * grad_kernel
+// the batch-reduced product with M = Cout, N = Kc = C * kH * kW, K = P = outH * outW per image: A = grad_output ([Cout][P] per
+// image, the op's aux laid out the same way), B = the images as a concatenated im2col source.  One chunk always, as for
+// batch_reduce_dev: chunks would round dW between them.
+int conv2d_filter_grad_dev(float *grad_kernel, const float *input, const ConvGeom &g, const float *grad_output, float alpha,
+                           float beta, const laser_b200_operand_op *op_in, int path, void *stream) {
+  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
+    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  OperandOp op;
+  const OperandOp *opA;
+  int rc;
+  if ((rc = operand_op_of(op_in, false, &op, &opA))) return rc;
+  const int64_t M = g.Cout, N = g.K(), P = g.outHW(), image = g.C * g.H * g.W;
+  if (opA && opA->aux && (opA->aux_sr != P || opA->aux_sc != 1))
+    return set_error(LASER_B200_EINVAL, "the aux tensor of op %d must be dense like grad_output: strides (%lld, 1), not (%lld, %lld)",
+                     opA->op, (long long)P, (long long)opA->aux_sr, (long long)opA->aux_sc);
+  if (g.B == 0) return LASER_B200_OK;
+  if (!grad_kernel || !input || !grad_output) return set_error(LASER_B200_EINVAL, "null pointer");
+  // B of a 1 x 1 kernel with unit strides and no padding is the images read in place: B_n[p][c] = input_n[c][p]
+  if (g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0) {
+    const laser_b200_batch_strides bs{M * P, image, 0, M * P, 0};
+    return batch_reduce_dev(g.B, M, N, P, alpha, grad_output, P, 1, input, 1, P, beta, grad_kernel, N, 1, &bs, opA, nullptr,
+                            Epilogue(), path, stream);
+  }
+  if (P > INT64_MAX / g.B) return set_error(LASER_B200_EUNSUPPORTED, "images * outH * outW overflows int64");
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  // PATH_AUTO decides as batch_reduce_dev does over K' = images * P (with an operand op: B is prepared, never the GEMV)
+  if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, g.B * P, Epilogue(), /*operand_op=*/true);
+  const BatchArgs bat{g.B, M * P, image, 0, M * P, 0, true};
+  if (path == LASER_B200_PATH_SIMT)
+    rc = batch_reduce_simt(*c, bat, M, N, P, alpha, grad_output, P, 1, input, 0, 0, beta, grad_kernel, N, 1, s, Epilogue(), opA,
+                           nullptr, &g);
+  else
+    rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, P, alpha, grad_output, P, 1, input, 0, 0, beta, grad_kernel, N, 1, s,
+                           Epilogue(), nullptr, opA, nullptr, &bat, &g);
+  if (rc) return rc;
   g_last_path = path;
   return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
@@ -1909,5 +1977,6 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 
 #define LB200_BATCHED_FUSED_F32 batched_fused_entry
 #define LB200_CONV2D_FUSED_F32 conv2d_fused_dev
+#define LB200_CONV2D_FILTER_GRAD_F32 conv2d_filter_grad_dev
 #include "capi_layers.inc"
 #include "capi_multi.inc"

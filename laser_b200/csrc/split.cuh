@@ -631,6 +631,87 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, fl
   }
 }
 
+// ---- concatenated im2col source: a convolution's filter-gradient B prepared straight from the NCHW images -------------
+// Tap row t = (c * kH + krow) * kW + kcol holds the tap's shifted input plane of every image of the launch, end to end:
+//   row[t][n * P + oh * outW + ow] = in[n][c][oh * sH - pH + krow][ow * sW - pW + kcol]   (0 outside the image), P = outHW
+// -- the images' im2col matrices [K][P] laid side by side, which is what the batch-reduce entry prepares from materialised
+// matrices read transposed (a K-major operand concatenated along k).  Each row is written in the format of the row kernel it
+// replaces over that concatenation, bit for bit (im2col_rows_kernel's modes):
+//   IM2COL_F32   the values, ld = round_up(n * P, 4)
+//   IM2COL_TF32  hi / lo as split_rows_tf32_kernel, ld = round_up(n * P, 4)
+//   IM2COL_F16X2 both fp16 pieces as f16x2_rows_fused_kernel against the row's abs-max word, ld = round_up(n * P, 8); the word
+//                comes from an ABSMAX launch of the same tiles first (words zeroed by the host, combined with atomicMax)
+// Every column up to ld is written (zeros past n * P).  The rows are few and very long (576 x 100352 floats for 32 images of
+// a 56 x 56, 64-channel layer), so a work item is a tile of TAP_SEG columns of one row: the tap is decoded once per tile, the
+// pixel once per float4, and adjacent threads take adjacent float4, so a warp reads consecutive ow -- consecutive addresses
+// when sW = 1.  Both passes read the images, which are small enough to stay in L2 between them.
+constexpr int TAP_VEC = 4;                     // float4 per thread of a tile
+constexpr int TAP_SEG = 256 * 4 * TAP_VEC;     // columns of one tile
+template <int MODE, bool ABSMAX = false>
+__global__ void __launch_bounds__(256)
+im2col_tap_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, float *__restrict__ dst, float *__restrict__ dst_lo,
+                       uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld, uint32_t *__restrict__ absmax) {
+  static_assert(!ABSMAX || MODE == IM2COL_F16X2, "only the f16x2 rows carry a scale word");
+  ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
+  const int64_t segs = (ld + TAP_SEG - 1) / TAP_SEG;
+  const int khw = q.kH * q.kW, HW = q.H * q.W;
+  const uint32_t P = static_cast<uint32_t>(q.outHW);
+  const int outH = static_cast<int>(q.outHW / q.outW);
+  for (int64_t it = blockIdx.x; it < q.K * segs; it += gridDim.x) {
+    const int t = static_cast<int>(it / segs);
+    const int64_t j0 = (it - t * segs) * TAP_SEG;
+    const int c = t / khw, kr = (t - c * khw) / q.kW, kc = t - c * khw - kr * q.kW;
+    const int64_t n0 = j0 / P;
+    const uint32_t p0 = static_cast<uint32_t>(j0 - n0 * P);                 // (p0 + d < 2^32: conv_geom bounds P by 2^31)
+    const float *plane0 = in + n0 * q.image + static_cast<int64_t>(c) * HW;   // channel c of image n0
+    float s = 1.0f;
+    if constexpr (MODE == IM2COL_F16X2 && !ABSMAX) s = f16x2_scale(absmax[t]);
+    uint32_t m = 0u;
+#pragma unroll
+    for (int i = 0; i < TAP_VEC; ++i) {
+      const uint32_t d = (static_cast<uint32_t>(threadIdx.x) + 256u * i) * 4u;   // this float4's column in the tile
+      if (j0 + d < ld) {
+        const uint32_t dn = (p0 + d) / P, p = p0 + d - dn * P;
+        int oh = static_cast<int>(p) / q.outW, ow = static_cast<int>(p) - oh * q.outW;
+        int64_t n = n0 + dn;
+        const float *plane = plane0 + dn * q.image;
+        float v[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int h = oh * q.sH - q.pH + kr, w = ow * q.sW - q.pW + kc;
+          const bool inside = n < images && static_cast<unsigned>(h) < static_cast<unsigned>(q.H) &&
+                              static_cast<unsigned>(w) < static_cast<unsigned>(q.W);
+          v[e] = inside ? plane[h * q.W + w] : 0.0f;
+          if (++ow == q.outW) { ow = 0; if (++oh == outH) { oh = 0; ++n; plane += q.image; } }
+        }
+        const float4 x = make_float4(v[0], v[1], v[2], v[3]);
+        const int64_t j = j0 + d;
+        if constexpr (ABSMAX) {
+          m = max(max(m, finite_abs_bits(x.x)), max(finite_abs_bits(x.y), max(finite_abs_bits(x.z), finite_abs_bits(x.w))));
+        } else if constexpr (MODE == IM2COL_F32) {
+          *reinterpret_cast<float4 *>(dst + t * ld + j) = x;
+        } else if constexpr (MODE == IM2COL_TF32) {
+          float4 h, l;
+          h.x = tf32_rna(x.x); l.x = tf32_lo(x.x, h.x);
+          h.y = tf32_rna(x.y); l.y = tf32_lo(x.y, h.y);
+          h.z = tf32_rna(x.z); l.z = tf32_lo(x.z, h.z);
+          h.w = tf32_rna(x.w); l.w = tf32_lo(x.w, h.w);
+          *reinterpret_cast<float4 *>(dst + t * ld + j) = h;
+          *reinterpret_cast<float4 *>(dst_lo + t * ld + j) = l;
+        } else {
+          store_f16x2_vec(x, s, hb + t * ld, lb + t * ld, j);
+        }
+      }
+    }
+    if constexpr (ABSMAX) {
+      float mf = __uint_as_float(m);     // non-negative finite: fmaxf orders them like the integers
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mf = fmaxf(mf, __shfl_xor_sync(0xffffffffu, mf, o));
+      if ((threadIdx.x & 31) == 0) atomicMax(absmax + t, __float_as_uint(mf));
+    }
+  }
+}
+
 // dst[r*ld + c] = src[r*sr + c*sc] for r < R, c < Cc.  32 x 32 tiles through shared
 // memory so that both the gather (along whichever source stride is smaller) and the
 // store (along c) are coalesced.  SPLIT: also write lo (fp32 only).

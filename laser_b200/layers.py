@@ -9,6 +9,8 @@
     im2col, conv2d_im2col                         conv2d_im2col.nim:44-166
     conv2d_fused                                  conv2d_im2col.nim:95-166 + bias + activation, im2col folded into the
                                                   GEMM's operand preparation (README.md:251)
+    conv2d_filter_grad_fused                      its filter gradient, derivative op on grad_output and the window gather
+                                                  folded into the operand preparation (README.md:244-245, :251)
     gemm_strided_batched                          (roadmap item of the reference, README.md:253-263)
     copyFrom(dst, src)                            laser/tensor/initialization.nim:80-112
 
@@ -19,14 +21,15 @@ import ctypes
 
 import numpy as np
 
-from ._capi import PATH_AUTO, Epilogue, check, lib
+from ._capi import OP_NAMES, PATH_AUTO, Epilogue, OperandOp, check, lib
 from .gemm import _current_stream, _resolve, _scalar
 from .tensor import _ITEMSIZE, Tensor
 
 FOREACH_OPS = {"copy": 0, "fill": 1, "scale": 2, "add": 3, "sub": 4, "mul": 5, "fma": 6, "axpy": 7, "bench": 8}
 
 __all__ = ["forEach", "FOREACH_OPS", "transpose2D_copy", "transpose2D_batched", "nchw2nhwc", "nhwc2nchw", "conv2d_out_shape",
-           "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "gemm_strided_batched", "copyFrom"]
+           "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "conv2d_filter_grad_fused", "gemm_strided_batched",
+           "copyFrom"]
 
 _i64 = ctypes.c_int64
 
@@ -144,6 +147,28 @@ def conv2d_fused(output, input, ishape, kernel, kshape, padding, strides, bias=N
     stream = _current_stream() if stream is None else stream
     check(lib().laser_b200_conv2d_f32_fused_dev(po, pi, _i4(ishape), pk, _i4(kshape), _i2(padding), _i2(strides),
                                                 ctypes.byref(epi), int(path), stream))
+
+
+def conv2d_filter_grad_fused(grad_kernel, input, ishape, grad_output, kshape, padding, strides, alpha=1.0, beta=0.0, op=None,
+                             aux=None, path=PATH_AUTO, stream=None):
+    """grad_kernel <- alpha * sum_n op(grad_output_n) * im2col(input_n)^T + beta * grad_kernel on float32 DEVICE buffers: the
+    filter gradient of conv2d_fused (input and grad_output dense NCHW, grad_kernel dense [c_out, c_in, kH, kW]).  op: None or
+    relu | tanh | sigmoid | relu_grad | tanh_grad | sigmoid_grad, applied to grad_output; a derivative takes `aux`, a dense
+    NCHW tensor of grad_output's shape (the forward output).  beta=1 accumulates across micro-batches.  One batch-reduced
+    product whose B operand is prepared straight from the images: no im2col matrix, no workspace."""
+    pw, pi, pg = _dev_f32(grad_kernel), _dev_f32(input), _dev_f32(grad_output)
+    o = None
+    if op is not None:
+        o = OperandOp()
+        o.op = OP_NAMES[op]
+        if aux is not None:
+            _, _, oh, ow = conv2d_out_shape(ishape, kshape, padding, strides)
+            o.aux = _dev_f32(aux)
+            o.auxRowStride, o.auxColStride = oh * ow, 1
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_filter_grad_f32_fused_dev(pw, pi, _i4(ishape), pg, _i4(kshape), _i2(padding), _i2(strides),
+                                                            float(alpha), float(beta), ctypes.byref(o) if o is not None else None,
+                                                            int(path), stream))
 
 
 def gemm_strided_batched(batch, M, N, K, alpha, A, rowStrideA, colStrideA, batchStrideA, B, rowStrideB, colStrideB,
