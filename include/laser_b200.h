@@ -479,6 +479,30 @@ int laser_b200_conv2d_filter_grad_f32_fused_dev(float *grad_kernel, const float 
                                                 const int64_t padding[2], const int64_t strides[2],
                                                 float alpha, float beta, const laser_b200_operand_op *op,
                                                 int path, void *stream);
+/* Input gradient of the fused convolution (the reference has no backward convolution):
+ *   grad_input <- alpha * conv_transpose(op(grad_output), kernel) + beta * grad_input
+ * with the forward call's shapes: grad_input dense NCHW of shape ishape, grad_output dense NCHW [n][c_out][outH][outW]
+ * (conv2d_out_shape), kernel dense [c_out][c_in][kH][kW].  op (NULL: none) is applied to grad_output, with the op set and aux
+ * rules of conv2d_filter_grad_f32_fused_dev (a derivative op's aux: dense NCHW of grad_output's shape, auxRowStride =
+ * outH * outW, auxColStride = 1) -- so the backward pass of a forward call with relu is this call and the filter-gradient
+ * call, both with LASER_B200_OP_RELU_GRAD and the forward output as aux.  beta = 1 accumulates into an existing gradient
+ * (e.g. where a residual branch joins).  No bias gradient.
+ *   Per image, grad_input_n = W' * B_n, the forward call's product over another B: W'[ci][(co, kh', kw')] =
+ *   kernel[co][ci][kH-1-kh'][kW-1-kw'] (written once per call into library workspace) and row ih * W + iw of B_n the input
+ *   pixel's window over grad_output_n zero-dilated by the strides and padded by kH - 1 - pH, in the forward im2col order, 0
+ *   where a tap falls between, before or past the output gradient's rows and columns (input rows and columns no window
+ *   covers get beta * grad_input only).  B is prepared straight from grad_output, the images of a chunk
+ *   (LASER_B200_BATCH_WS_MB) share one GEMM launch, and at stride 1 with pH <= kH - 1 grad_input is bit for bit
+ *   conv2d_f32_fused_dev over (grad_output, W', padding kH - 1 - pH) on the same path.  1 x 1 kernels with unit strides and
+ *   no padding are the batched fused product kernel^T * grad_output_n, with grad_output read in place.
+ *   PATH_AUTO decides as conv2d_f32_fused_dev does for M = c_in, N = H * W, K' = c_out * kH * kW.
+ *   n = 0: LASER_B200_OK, nothing launched.  K' must fit in int32 (LASER_B200_EUNSUPPORTED otherwise).
+ *   LASER_B200_EINVAL, before anything is launched: geometry errors, kshape[1] != c_in, an unknown path or op, a derivative
+ *   op without aux or with other aux strides, a NULL pointer. */
+int laser_b200_conv2d_input_grad_f32_fused_dev(float *grad_input, const int64_t ishape[4], const float *grad_output,
+                                               const float *kernel, const int64_t kshape[4], const int64_t padding[2],
+                                               const int64_t strides[2], float alpha, float beta,
+                                               const laser_b200_operand_op *op, int path, void *stream);
 /* host pointers, synchronous, library-owned workspace */
 int laser_b200_conv2d_im2col_f32(float *output, const float *input, const int64_t ishape[4],
                                  const float *kernel, const int64_t kshape[4], const int64_t padding[2],

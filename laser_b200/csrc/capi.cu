@@ -128,6 +128,7 @@ struct Ctx {
   Buffer splitk;     // split-K partial-sum planes
   Buffer bpanels;    // row-sharded products: B prepared, panel-major (capi_multi.inc: rowshard_prepared)
   Buffer layer_ws;   // im2col workspace of the host-pointer convolution
+  Buffer tfilt;      // the convolution input gradient's rotated filters W' (conv2d_input_grad_dev), under tfilt_mu for a whole call
   Buffer f16s;       // F16X3 mode: fp32 bits of max_k |a| per row of A (words [0, M)) and of max_k |b| per column of B (from
                      // f16_b_off on), written and read on the device
   Buffer sched;      // kSchedSlots x {next unit, CTAs done}: the kernel re-zeroes its slot when it ends
@@ -135,6 +136,7 @@ struct Ctx {
   cudaEvent_t ws_free = nullptr;  // recorded after the last kernel that reads ws[]
   std::mutex mu;       // workspace + tensor-map construction
   std::mutex host_mu;  // staging buffers of the host-pointer entry points
+  std::mutex tfilt_mu; // tfilt: written once per input-gradient call, read by every chunk's product (each takes mu itself)
   std::atomic<bool> ready{false};
 };
 
@@ -579,21 +581,42 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
 // the format of `mode` -- words and fp16 pieces into hb / lb / words (F16X2), tf32 hi / lo into dst / dst_lo (TF32), the
 // values into dst (NONE: TF32X1 and the exact path).  A concatenated one (with Operand::concat): the tap rows [mn][ld] of
 // every image end to end (split.cuh: im2col_tap_rows_kernel), F16X2 after an abs-max pass over the same tiles.
+// A dilated source (ConvGeom::dH, dW) or an op: the transposed source of the input gradient, the rows kernel's DIL / HAS_OP
+// instantiations (op applied to the values read, its aux dense like the images; not with `concat`).
 int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst_lo, uint16_t *hb, uint16_t *lb, int64_t ld,
-                uint32_t *words, cudaStream_t s) {
+                uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
   const Im2colSrc q = im2col_src(*o.conv);
   const int64_t images = batch_of(o).n, rows = images * o.mn;
   const int64_t tiles = o.mn * ((ld + TAP_SEG - 1) / TAP_SEG);
   const float *in = static_cast<const float *>(o.ptr);
+  const bool dil = o.conv->dH != 1 || o.conv->dW != 1;
+  if (o.concat && (dil || op)) return set_error(LASER_B200_ECUDA, "internal: a concatenated im2col source has no dilation or op");
   auto launch = [&](auto m, auto absmax) {
     constexpr int MODE = decltype(m)::value, PER_SM = MODE == IM2COL_F16X2 ? 3 : 4;   // the kernel's launch bounds
-    if (o.concat)
+    auto rows_kernel = [&](auto d, auto has_op, const auto &src) {
+      constexpr bool DIL = decltype(d)::value, HAS_OP = decltype(has_op)::value;
+      if (ld <= 4 * 32 * F16ROWS_MAXV)
+        im2col_rows_kernel<MODE, 32, DIL, HAS_OP><<<grid_for(c, (rows + 7) / 8, PER_SM), 256, 0, s>>>(in, src, images, dst, dst_lo, hb,
+                                                                                                   lb, ld, words);
+      else
+        im2col_rows_kernel<MODE, 256, DIL, HAS_OP><<<grid_for(c, rows, PER_SM), 256, 0, s>>>(in, src, images, dst, dst_lo, hb, lb, ld,
+                                                                                          words);
+    };
+    if (o.concat) {
       im2col_tap_rows_kernel<MODE, decltype(absmax)::value><<<grid_for(c, tiles, 8), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb,
                                                                                                  ld, words);
-    else if (ld <= 4 * 32 * F16ROWS_MAXV)
-      im2col_rows_kernel<MODE, 32><<<grid_for(c, (rows + 7) / 8, PER_SM), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb, ld, words);
-    else
-      im2col_rows_kernel<MODE, 256><<<grid_for(c, rows, PER_SM), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb, ld, words);
+    } else if (dil || op) {
+      Im2colGradSrc gq{};
+      static_cast<Im2colSrc &>(gq) = q;
+      gq.dH = static_cast<int>(o.conv->dH);
+      gq.dW = static_cast<int>(o.conv->dW);
+      if (op) gq.op = *op;
+      if (dil && op) rows_kernel(std::true_type(), std::true_type(), gq);
+      else if (dil) rows_kernel(std::true_type(), std::false_type(), gq);
+      else rows_kernel(std::false_type(), std::true_type(), gq);
+    } else {
+      rows_kernel(std::false_type(), std::false_type(), q);
+    }
     COUNT_LAUNCH();
     CHECK_LAUNCH();
     return LASER_B200_OK;
@@ -627,7 +650,7 @@ int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst
 template <int ESZ>
 int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w, int block_mn,
                     OperandMaps *m, bool *used_ws, cudaStream_t s, const OperandOp *op = nullptr) {
-  const bool conv = o.conv != nullptr;   // (fp32, no op)
+  const bool conv = o.conv != nullptr;   // (fp32; its op is applied by the rows kernel as it reads the source)
   const Major mj = conv ? K_MAJOR : classify(o, ESZ);
   const Batch bt = batch_of(o);
   const bool cat = o.concat;
@@ -671,7 +694,7 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
       uint16_t *hb = static_cast<uint16_t *>(w.p0->ptr), *lb = static_cast<uint16_t *>(w.p1->ptr);
       uint32_t *words = static_cast<uint32_t *>(c.f16s.ptr) + w.amax_off;
       if (conv) {
-        rc = im2col_rows(c, o, mode, nullptr, nullptr, hb, lb, ld_b, words, s);
+        rc = im2col_rows(c, o, mode, nullptr, nullptr, hb, lb, ld_b, words, s, op);
       } else if (!in_place) {   // the gathered problems are stacked (concatenated) rows: one plain row pass over all of them
         if ((rc = gather<float>(c, o, *w.gather, nullptr, s, op))) return rc;
         rc = f16x2_rows(c, static_cast<const float *>(w.gather->ptr), rows_p, row_len, ld, hb, lb, ld_b, words, s);
@@ -692,7 +715,7 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
       if ((rc = ensure(*w.p0, bytes))) return rc;
       if (mode == SPLIT_TF32 && (rc = ensure(*w.p1, bytes))) return rc;
       float *p0 = static_cast<float *>(w.p0->ptr), *p1 = mode == SPLIT_TF32 ? static_cast<float *>(w.p1->ptr) : nullptr;
-      rc = conv ? im2col_rows(c, o, mode, p0, p1, nullptr, nullptr, ld, nullptr, s)
+      rc = conv ? im2col_rows(c, o, mode, p0, p1, nullptr, nullptr, ld, nullptr, s, op)
                 : tf32_split(c, src, R, Cc, src_ld, p0, p1, ld, s, on_load, bt, cat);
     }
     if (rc) return rc;
@@ -1327,9 +1350,10 @@ int batch_reduce_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha
 // ---------------------------------------------------------------------------------------
 //     fused convolution: im2col folded into the preparation of B, the images of a chunk in one GEMM launch
 // ---------------------------------------------------------------------------------------
-// Exact path, `images` images: their windows as plain K-major rows in the gather workspace, one batched exact-kernel launch
-int conv2d_simt(Ctx &c, const ConvGeom &g, int64_t images, const float *kernel, const float *input, float *output, cudaStream_t s,
-                const Epilogue &epi) {
+// Exact path, `images` images: their windows as plain K-major rows in the gather workspace (opB applied), one batched
+// exact-kernel launch with A = [Cout][K] rows lda apart
+int conv2d_simt(Ctx &c, const ConvGeom &g, int64_t images, float alpha, const float *A, int64_t lda, const float *input, float beta,
+                float *output, cudaStream_t s, const Epilogue &epi, const OperandOp *opB) {
   const int64_t M = g.Cout, K = g.K(), N = g.outHW(), ld = round_up(K, 4);
   std::lock_guard<std::mutex> lk(c.mu);   // the gather buffer is workspace
   CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
@@ -1338,33 +1362,29 @@ int conv2d_simt(Ctx &c, const ConvGeom &g, int64_t images, const float *kernel, 
   Operand o{input, N, K, 0, 0, images, g.C * g.H * g.W};
   o.conv = &g;
   float *rows = static_cast<float *>(c.gather[1].ptr);
-  if ((rc = im2col_rows(c, o, SPLIT_NONE, rows, nullptr, nullptr, nullptr, ld, nullptr, s))) return rc;
-  if ((rc = gemm_simt<float>(c, M, N, K, 1.0f, kernel, K, 1, rows, 1, ld, 0.0f, output, N, 1, s, epi, images, 0, N * ld, M * N)))
+  if ((rc = im2col_rows(c, o, SPLIT_NONE, rows, nullptr, nullptr, nullptr, ld, nullptr, s, opB))) return rc;
+  if ((rc = gemm_simt<float>(c, M, N, K, alpha, A, lda, 1, rows, 1, ld, beta, output, N, 1, s, epi, images, 0, N * ld, M * N)))
     return rc;
   CUDA_TRY(cudaEventRecord(c.ws_free, s));
   return LASER_B200_OK;
 }
 
-// laser_b200_conv2d_f32_fused_dev (capi_layers.inc checks the geometry): output_n = act(F * im2col(input_n) + bias) for every
-// image n.  A = the filters F [Cout][K], shared by the images (prepared once per launch); B = the images as an im2col source.
-int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const float *kernel, const laser_b200_epilogue *epi_in,
-                     int path, void *stream) {
-  Epilogue epi;
+// The product of both fused convolution entries, image by image: output_n = epi(alpha * A * B_n + beta * output_n), A [Cout][K]
+// (rsA, csA; K-major with 16-byte rows unless the kernel is 1 x 1), shared by the images; B_n image n of `input` as an im2col
+// source of geometry g (dilated: ConvGeom::dH, dW), opB applied to its values (aux dense like `input`).  Chunks of whole
+// images under LASER_B200_BATCH_WS_MB: the images do not sum into each other.
+int conv_windows_dev(const ConvGeom &g, float alpha, const float *A, int64_t rsA, int64_t csA, const float *input, float beta,
+                     float *output, const OperandOp *opB, const Epilogue &epi, int path, void *stream) {
   int rc;
-  if ((rc = epilogue_of(epi_in, &epi))) return rc;
-  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
-    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
-  if (g.B == 0) return LASER_B200_OK;
-  if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
   const int64_t M = g.Cout, K = g.K(), N = g.outHW(), image = g.C * g.H * g.W;
   // PATH_AUTO decides as conv2d_im2col_f32_dev does: the exact kernel for a batch of short M or K (batched_f32_dev), else
   // resolve_auto with this call's epilogue (never the GEMV: N is a pixel count and the batch needs one launch)
   if (path == LASER_B200_PATH_AUTO)
     path = (g.B > 1 && (M < 64 || K < 64)) ? LASER_B200_PATH_SIMT : resolve_auto(M, N, K, epi, /*operand_op=*/true);
-  if (g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0) {   // the image already is the [C][H*W] matrix
-    const laser_b200_batch_strides bs{0, image, M * N, 0, 0};
-    return batched_fused_dev(g.B, M, N, K, 1.0f, kernel, K, 1, input, N, 1, 0.0f, output, N, 1, &bs, nullptr, nullptr, epi, path,
-                             stream);
+  if (g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0 && g.dH == 1 && g.dW == 1) {
+    // the image already is the [C][H*W] matrix
+    const laser_b200_batch_strides bs{0, image, M * N, 0, image};
+    return batched_fused_dev(g.B, M, N, K, alpha, A, rsA, csA, input, N, 1, beta, output, N, 1, &bs, nullptr, opB, epi, path, stream);
   }
   Ctx *c;
   if ((rc = get_ctx(&c))) return rc;
@@ -1379,17 +1399,87 @@ int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const
     const int64_t cnt = g.B - n0 < chunk ? g.B - n0 : chunk;
     const float *in = input + n0 * image;
     float *out = output + n0 * M * N;
+    OperandOp ob;
+    if (opB) { ob = *opB; if (ob.aux) ob.aux += n0 * image; }
     if (path == LASER_B200_PATH_SIMT) {
-      rc = conv2d_simt(*c, g, cnt, kernel, in, out, s, epi);
+      rc = conv2d_simt(*c, g, cnt, alpha, A, rsA, in, beta, out, s, epi, opB ? &ob : nullptr);
     } else {
-      const BatchArgs bat{cnt, 0, image, M * N, 0, 0};
-      rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, 1.0f, kernel, K, 1, in, 0, 0, 0.0f, out, N, 1, s, epi, nullptr, nullptr,
-                             nullptr, &bat, &g);
+      const BatchArgs bat{cnt, 0, image, M * N, 0, image};
+      rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, in, 0, 0, beta, out, N, 1, s, epi, nullptr, nullptr,
+                             opB ? &ob : nullptr, &bat, &g);
     }
     if (rc) return rc;
   }
   g_last_path = path;
   return finish(*c, static_cast<cudaStream_t>(stream), s);
+}
+
+// laser_b200_conv2d_f32_fused_dev (capi_layers.inc checks the geometry): output_n = act(F * im2col(input_n) + bias) for every
+// image n.  A = the filters F [Cout][K], shared by the images (prepared once per launch); B = the images as an im2col source.
+int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const float *kernel, const laser_b200_epilogue *epi_in,
+                     int path, void *stream) {
+  Epilogue epi;
+  int rc;
+  if ((rc = epilogue_of(epi_in, &epi))) return rc;
+  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
+    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  if (g.B == 0) return LASER_B200_OK;
+  if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
+  return conv_windows_dev(g, 1.0f, kernel, g.K(), 1, input, 0.0f, output, nullptr, epi, path, stream);
+}
+
+template <typename T>
+int launch_copy(Ctx &c, void *dst, const void *src, const CopyParams &p, cudaStream_t s);   // capi_layers.inc
+
+// ---------------------------------------------------------------------------------------
+//   convolution input gradient: the forward product over the output gradients as a transposed, dilated im2col source
+// ---------------------------------------------------------------------------------------
+// laser_b200_conv2d_input_grad_f32_fused_dev (capi_layers.inc checks the geometry):
+//   grad_input_n <- alpha * W' * B_n + beta * grad_input_n,  W'[ci][(co, kh', kw')] = W[co][ci][kH-1-kh'][kW-1-kw']
+// B_n: grad_output_n (op applied) as the im2col source of the transposed geometry gt -- C = Cout, H x W = outH x outW,
+// padding kH - 1 - pH, stride 1, dilated by the forward strides, windows at the input's H x W pixels (split.cuh:
+// Im2colGradSrc).  M = C, N = H * W, K' = Cout * kH * kW; conv_windows_dev runs it as it runs the forward call.
+int conv2d_input_grad_dev(float *grad_input, const ConvGeom &g, const float *grad_output, const float *kernel, float alpha, float beta,
+                          const laser_b200_operand_op *op_in, int path, void *stream) {
+  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
+    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  OperandOp op;
+  const OperandOp *opB;
+  int rc;
+  if ((rc = operand_op_of(op_in, true, &op, &opB))) return rc;
+  const int64_t P = g.outHW(), khw = g.kH * g.kW;
+  // (B seen as [mn = pixel][k = channel]: a dense NCHW aux has aux_sr = 1, aux_sc = outH * outW)
+  if (opB && opB->aux && (opB->aux_sr != 1 || opB->aux_sc != P))
+    return set_error(LASER_B200_EINVAL, "the aux tensor of op %d must be dense like grad_output: strides (%lld, 1), not (%lld, %lld)",
+                     opB->op, (long long)P, (long long)opB->aux_sc, (long long)opB->aux_sr);
+  if (g.B == 0) return LASER_B200_OK;
+  if (!grad_input || !grad_output || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
+  if (g.Cout > INT32_MAX / khw) return set_error(LASER_B200_EUNSUPPORTED, "c_out * kH * kW beyond 2^31");
+  ConvGeom gt = g;
+  gt.C = g.Cout; gt.H = g.outH; gt.W = g.outW; gt.Cout = g.C;
+  gt.pH = g.kH - 1 - g.pH; gt.pW = g.kW - 1 - g.pW;
+  gt.sH = gt.sW = 1;
+  gt.dH = g.sH; gt.dW = g.sW;
+  gt.outH = g.H; gt.outW = g.W;
+  const int64_t K = gt.K();
+  // dX_n = W^T * dY_n for a 1 x 1 kernel with unit strides and no padding: W read transposed, no copy
+  if (khw == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0)
+    return conv_windows_dev(gt, alpha, kernel, 1, g.C, grad_output, beta, grad_input, opB, Epilogue(), path, stream);
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  // W' once per call into library workspace, K-major rows 16 bytes apart, read in place by every chunk's product.  The buffer
+  // is this entry's alone, held for the whole call; the copy waits for the last kernel that read it (ws_free).
+  std::lock_guard<std::mutex> lk(c->tfilt_mu);
+  const int64_t lda = round_up(K, 4);
+  if ((rc = ensure(c->tfilt, static_cast<size_t>(g.C * lda) * sizeof(float)))) return rc;
+  CUDA_TRY(cudaStreamWaitEvent(s, c->ws_free, 0));
+  const int64_t shape[4] = {g.C, g.Cout, g.kH, g.kW}, dst_st[4] = {lda, khw, g.kW, 1}, src_st[4] = {khw, g.C * khw, -g.kW, -1};
+  CopyParams cp;
+  copy_plan(4, shape, dst_st, src_st, &cp);
+  float *wt = static_cast<float *>(c->tfilt.ptr);
+  if ((rc = launch_copy<uint32_t>(*c, wt, kernel + khw - 1, cp, s))) return rc;
+  return conv_windows_dev(gt, alpha, wt, lda, 1, grad_output, beta, grad_input, opB, Epilogue(), path, stream);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1644,6 +1734,7 @@ void laser_b200_shutdown(void) {
     if (c.splitk.ptr) { cudaFree(c.splitk.ptr); c.splitk = Buffer(); }
     if (c.bpanels.ptr) { cudaFree(c.bpanels.ptr); c.bpanels = Buffer(); }
     if (c.layer_ws.ptr) { cudaFree(c.layer_ws.ptr); c.layer_ws = Buffer(); }
+    if (c.tfilt.ptr) { cudaFree(c.tfilt.ptr); c.tfilt = Buffer(); }
     if (c.f16s.ptr) { cudaFree(c.f16s.ptr); c.f16s = Buffer(); }
     for (auto &b : c.gather) { if (b.ptr) cudaFree(b.ptr); b = Buffer(); }
     if (c.sched.ptr) { cudaFree(c.sched.ptr); c.sched = Buffer(); }
@@ -1978,5 +2069,6 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 #define LB200_BATCHED_FUSED_F32 batched_fused_entry
 #define LB200_CONV2D_FUSED_F32 conv2d_fused_dev
 #define LB200_CONV2D_FILTER_GRAD_F32 conv2d_filter_grad_dev
+#define LB200_CONV2D_INPUT_GRAD_F32 conv2d_input_grad_dev
 #include "capi_layers.inc"
 #include "capi_multi.inc"

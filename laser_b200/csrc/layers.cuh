@@ -86,6 +86,9 @@ transpose_batched_kernel(T *__restrict__ dst, const T *__restrict__ src, int64_t
 // ---- convolution geometry (conv2d_common.nim:6-45): NCHW images, [Cout][C][kH][kW] filters ----
 struct ConvGeom {
   int64_t B, C, H, W, Cout, kH, kW, pH, pW, sH, sW, outH, outW;
+  // dilation of the source (an im2col source only): the transposed geometry of the input gradient reads the output gradient
+  // zero-dilated by the forward strides (split.cuh: Im2colGradSrc)
+  int64_t dH = 1, dW = 1;
   __host__ __device__ int64_t K() const { return C * kH * kW; }
   __host__ __device__ int64_t outHW() const { return outH * outW; }
 };

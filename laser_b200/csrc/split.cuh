@@ -17,6 +17,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "f16_scale.cuh"
 #include "layers.cuh"
 #include "ptx.cuh"
@@ -556,11 +558,71 @@ __device__ __forceinline__ float4 window_vec(const float *__restrict__ img, cons
   }
   return make_float4(v[0], v[1], v[2], v[3]);
 }
+
+// ---- transposed source: a convolution's input gradient, B prepared straight from the output gradients --------------
+// The input gradient dX_n = W' * B_n is the forward product over another source (W': the filters rotated by 180 degrees, the
+// channel axes swapped).  Row ih * W + iw of B_n is input pixel (ih, iw)'s window over the output gradient dY_n, zero-dilated
+// by the forward strides, padded by kH - 1 - pH (which may be negative) and windowed at stride 1, in the forward im2col
+// order (co, kh', kw'): the forward windows with Im2colSrc's geometry over dY (C = c_out, H x W = outH x outW, pH = kH - 1 -
+// pH, sH = sW = 1, outW = the input's W, outHW = its H * W), read where the dilated position is a source value:
+//   h = ih - p' + kh' in the dilated plane; a source row when h >= 0, h % dH == 0 and h / dH < outH (columns likewise)
+// Everything else is a structural zero -- also the input rows and columns no window covers, (H + 2pH - kH) mod sH of them.
+// HAS_OP applies the operand op to the values read (aux at the same NCHW offset as the dY element); holes stay 0, never op(0).
+// A parameter struct of its own, so that Im2colSrc -- and every forward instantiation -- keeps its layout.
+struct Im2colGradSrc : Im2colSrc {
+  int dH, dW;     // source dilation: the forward strides (1: none)
+  OperandOp op;   // HAS_OP: the op on the source values
+};
+template <bool GRAD>
+using Im2colSrcOf = typename std::conditional<GRAD, Im2colGradSrc, Im2colSrc>::type;
+// elements k .. k+3 of the transposed window of pixel (oh, ow) of image `img` (aux: its aux image, HAS_OP)
+template <bool DIL, bool HAS_OP>
+__device__ __forceinline__ float4 grad_window_vec(const float *__restrict__ img, const float *__restrict__ aux, const Im2colGradSrc &q,
+                                                  int oh, int ow, int k) {
+  const int khw = q.kH * q.kW;
+  int c = k / khw;
+  int kr = (k - c * khw) / q.kW;
+  int kc = k - c * khw - kr * q.kW;
+  float v[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    int h = oh * q.sH - q.pH + kr, w = ow * q.sW - q.pW + kc;
+    bool inside = k + e < q.K;
+    if constexpr (DIL) {   // h >= 0 is tested, and the quotient used, before any remainder of a negative h could matter
+      const unsigned hq = static_cast<unsigned>(h) / static_cast<unsigned>(q.dH), wq = static_cast<unsigned>(w) / static_cast<unsigned>(q.dW);
+      inside = inside && h >= 0 && w >= 0 && hq * q.dH == static_cast<unsigned>(h) && wq * q.dW == static_cast<unsigned>(w) &&
+               hq < static_cast<unsigned>(q.H) && wq < static_cast<unsigned>(q.W);
+      h = static_cast<int>(hq);
+      w = static_cast<int>(wq);
+    } else {
+      inside = inside && static_cast<unsigned>(h) < static_cast<unsigned>(q.H) && static_cast<unsigned>(w) < static_cast<unsigned>(q.W);
+    }
+    float x = 0.0f;
+    if (inside) {
+      const int64_t off = (static_cast<int64_t>(c) * q.H + h) * q.W + w;
+      x = img[off];
+      if constexpr (HAS_OP) x = operand_op(q.op.op, x, aux ? aux[off] : 0.0f);
+    }
+    v[e] = x;
+    if (++kc == q.kW) { kc = 0; if (++kr == q.kH) { kr = 0; ++c; } }
+  }
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+template <bool DIL, bool HAS_OP, typename Src>
+__device__ __forceinline__ float4 source_vec(const float *__restrict__ img, const float *__restrict__ aux, const Src &q, int oh, int ow,
+                                             int k) {
+  if constexpr (DIL || HAS_OP) return grad_window_vec<DIL, HAS_OP>(img, aux, q, oh, ow, k);
+  else return window_vec(img, q, oh, ow, k);
+}
+
 // (F16X2: the row in registers next to the geometry needs more than the 64 registers of 4 CTAs per SM -- it spills there)
-template <int MODE, int GROUP>
+// DIL / HAS_OP (an Im2colGradSrc): the transposed source of the input gradient, dilated / with an op; the forward call's
+// instantiations are <MODE, GROUP, false, false>.
+template <int MODE, int GROUP, bool DIL = false, bool HAS_OP = false>
 __global__ void __launch_bounds__(256, MODE == IM2COL_F16X2 ? 3 : 4)
-im2col_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, float *__restrict__ dst, float *__restrict__ dst_lo,
-                   uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld, uint32_t *__restrict__ absmax) {
+im2col_rows_kernel(const float *__restrict__ in, Im2colSrcOf<DIL || HAS_OP> q, int64_t images, float *__restrict__ dst,
+                   float *__restrict__ dst_lo, uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld,
+                   uint32_t *__restrict__ absmax) {
   static_assert(GROUP == 32 || GROUP == 256, "a warp or the CTA per row");
   __shared__ uint32_t red[2][8];
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
@@ -576,9 +638,11 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, fl
     const int p = static_cast<int>(r - n * q.outHW);
     const int oh = p / q.outW, ow = p - oh * q.outW;
     const float *img = in + n * q.image;
+    const float *aux = nullptr;
+    if constexpr (HAS_OP) aux = q.op.aux ? q.op.aux + n * q.image : nullptr;
     if constexpr (MODE != IM2COL_F16X2) {
       for (int idx = tid; idx < nvec; idx += GROUP) {
-        const float4 v = window_vec(img, q, oh, ow, idx << 2);
+        const float4 v = source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2);
         if constexpr (MODE == IM2COL_F32) {
           *reinterpret_cast<float4 *>(dst + r * ld + (idx << 2)) = v;
         } else {
@@ -598,12 +662,12 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, fl
       for (int i = 0; i < F16ROWS_MAXV; ++i) {
         const int idx = tid + i * GROUP;
         if (idx < nvec) {
-          v[i] = window_vec(img, q, oh, ow, idx << 2);
+          v[i] = source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2);
           m = max(max(m, finite_abs_bits(v[i].x)), max(finite_abs_bits(v[i].y), max(finite_abs_bits(v[i].z), finite_abs_bits(v[i].w))));
         }
       }
       for (int idx = tid + F16ROWS_MAXV * GROUP; idx < nvec; idx += GROUP) {
-        const float4 t = window_vec(img, q, oh, ow, idx << 2);
+        const float4 t = source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2);
         m = max(max(m, finite_abs_bits(t.x)), max(finite_abs_bits(t.y), max(finite_abs_bits(t.z), finite_abs_bits(t.w))));
       }
       float mf = __uint_as_float(m);     // non-negative finite: fmaxf orders them like the integers
@@ -626,7 +690,7 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images, fl
         if (idx < nvec) store_f16x2_vec(v[i], s, hrow, lrow, static_cast<int64_t>(idx) << 2);
       }
       for (int idx = tid + F16ROWS_MAXV * GROUP; idx < nvec; idx += GROUP)
-        store_f16x2_vec(window_vec(img, q, oh, ow, idx << 2), s, hrow, lrow, static_cast<int64_t>(idx) << 2);
+        store_f16x2_vec(source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2), s, hrow, lrow, static_cast<int64_t>(idx) << 2);
     }
   }
 }

@@ -11,6 +11,8 @@
                                                   GEMM's operand preparation (README.md:251)
     conv2d_filter_grad_fused                      its filter gradient, derivative op on grad_output and the window gather
                                                   folded into the operand preparation (README.md:244-245, :251)
+    conv2d_input_grad_fused                       its input gradient, the transposed window gather over grad_output folded
+                                                  into the operand preparation
     gemm_strided_batched                          (roadmap item of the reference, README.md:253-263)
     copyFrom(dst, src)                            laser/tensor/initialization.nim:80-112
 
@@ -28,8 +30,8 @@ from .tensor import _ITEMSIZE, Tensor
 FOREACH_OPS = {"copy": 0, "fill": 1, "scale": 2, "add": 3, "sub": 4, "mul": 5, "fma": 6, "axpy": 7, "bench": 8}
 
 __all__ = ["forEach", "FOREACH_OPS", "transpose2D_copy", "transpose2D_batched", "nchw2nhwc", "nhwc2nchw", "conv2d_out_shape",
-           "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "conv2d_filter_grad_fused", "gemm_strided_batched",
-           "copyFrom"]
+           "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "conv2d_filter_grad_fused", "conv2d_input_grad_fused",
+           "gemm_strided_batched", "copyFrom"]
 
 _i64 = ctypes.c_int64
 
@@ -169,6 +171,28 @@ def conv2d_filter_grad_fused(grad_kernel, input, ishape, grad_output, kshape, pa
     check(lib().laser_b200_conv2d_filter_grad_f32_fused_dev(pw, pi, _i4(ishape), pg, _i4(kshape), _i2(padding), _i2(strides),
                                                             float(alpha), float(beta), ctypes.byref(o) if o is not None else None,
                                                             int(path), stream))
+
+
+def conv2d_input_grad_fused(grad_input, ishape, grad_output, kernel, kshape, padding, strides, alpha=1.0, beta=0.0, op=None,
+                            aux=None, path=PATH_AUTO, stream=None):
+    """grad_input <- alpha * conv_transpose(op(grad_output), kernel) + beta * grad_input on float32 DEVICE buffers: the input
+    gradient of conv2d_fused (grad_input dense NCHW of shape ishape, grad_output dense NCHW, kernel dense [c_out, c_in, kH,
+    kW]).  op and aux as for conv2d_filter_grad_fused, applied to grad_output.  beta=1 accumulates into an existing gradient.
+    The forward call's product over the filters rotated by 180 degrees and a B operand prepared straight from grad_output
+    (zero-dilated by the strides): no col2im, no workspace argument."""
+    pg, po, pk = _dev_f32(grad_input), _dev_f32(grad_output), _dev_f32(kernel)
+    o = None
+    if op is not None:
+        o = OperandOp()
+        o.op = OP_NAMES[op]
+        if aux is not None:
+            _, _, oh, ow = conv2d_out_shape(ishape, kshape, padding, strides)
+            o.aux = _dev_f32(aux)
+            o.auxRowStride, o.auxColStride = oh * ow, 1
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_input_grad_f32_fused_dev(pg, _i4(ishape), po, pk, _i4(kshape), _i2(padding), _i2(strides),
+                                                           float(alpha), float(beta), ctypes.byref(o) if o is not None else None,
+                                                           int(path), stream))
 
 
 def gemm_strided_batched(batch, M, N, K, alpha, A, rowStrideA, colStrideA, batchStrideA, B, rowStrideB, colStrideB,

@@ -294,6 +294,12 @@ proc laser_b200_conv2d_filter_grad_f32_fused_dev*(grad_kernel, input: ptr float3
                                                   grad_output: ptr float32, kshape: ptr array[4, int64],
                                                   padding, strides: ptr array[2, int64], alpha, beta: float32,
                                                   op: ptr LaserB200OperandOp, path: cint, stream: pointer): cint
+# its input gradient: grad_input <- alpha * conv_transpose(op(grad_output), kernel) + beta * grad_input, the forward product
+# over the rotated filters and a B prepared from grad_output; nil op = none
+proc laser_b200_conv2d_input_grad_f32_fused_dev*(grad_input: ptr float32, ishape: ptr array[4, int64],
+                                                 grad_output, kernel: ptr float32, kshape: ptr array[4, int64],
+                                                 padding, strides: ptr array[2, int64], alpha, beta: float32,
+                                                 op: ptr LaserB200OperandOp, path: cint, stream: pointer): cint
 {.pop.}
 
 proc transpose2D_copy*[T](dst, src: ptr (T or UncheckedArray[T]), NR, NC: Natural) =
