@@ -631,6 +631,21 @@ int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst
   return launch(std::integral_constant<int, IM2COL_F32>(), std::false_type());
 }
 
+// An fp32 operand as compact K-major rows [rows][round_up(k, 4)] (concatenated: [mn][round_up(batch * k, 4)]) in dst: gathered
+// from any strides with op applied, or an im2col source's windows.  SPLIT_TF32: the tf32 hi / lo pieces into dst / *lo,
+// SPLIT_NONE: the values (TF32X1 and the exact path).
+int f32_rows(Ctx &c, const Operand &o, SplitMode mode, Buffer &dst, Buffer *lo, cudaStream_t s, const OperandOp *op) {
+  if (!o.conv) return mode == SPLIT_TF32 ? gather<float, 1>(c, o, dst, lo, s, op) : gather<float>(c, o, dst, nullptr, s, op);
+  const Batch bt = batch_of(o);
+  const int64_t ld = round_up(o.concat ? bt.n * o.k : o.k, 4);
+  const size_t bytes = static_cast<size_t>((o.concat ? 1 : bt.n) * o.mn) * ld * sizeof(float);
+  int rc;
+  if ((rc = ensure(dst, bytes))) return rc;
+  if (mode == SPLIT_TF32 && (rc = ensure(*lo, bytes))) return rc;
+  return im2col_rows(c, o, mode, static_cast<float *>(dst.ptr), mode == SPLIT_TF32 ? static_cast<float *>(lo->ptr) : nullptr,
+                     nullptr, nullptr, ld, nullptr, s, op);
+}
+
 // One operand of a tensor-core call: first the plan, then its steps.
 //   An im2col source: one pass from the images into the prepared rows, K-major like a gathered operand.
 //   A concatenated im2col source: the tap rows of every image end to end, K-major [mn][batch * k] (F16X3: an abs-max pass
@@ -708,15 +723,13 @@ int prepare_operand(Ctx &c, const Operand &o, SplitMode mode, const OperandWs &w
       if ((rc = operand_map(c, &m->p0, 2, w.p0->ptr, out_mj, o.mn, kk, ld_b, block_mn, depth, d_stride(ld_b)))) return rc;
       return operand_map(c, &m->p1, 2, w.p1->ptr, out_mj, o.mn, kk, ld_b, block_mn, depth, d_stride(ld_b));
     }
-    if (!in_place && !conv) {
-      rc = (mode == SPLIT_TF32) ? gather<float, 1>(c, o, *w.p0, w.p1, s, op) : gather<float>(c, o, *w.p0, nullptr, s, op);
-    } else {   // TF32X3 K-major, or an im2col source (TF32X3, TF32X1)
+    if (!in_place || conv) {
+      rc = f32_rows(c, o, mode, *w.p0, w.p1, s, op);
+    } else {   // TF32X3 K-major: the split reads the caller's memory
       const size_t bytes = static_cast<size_t>(rows_p) * ld * sizeof(float);
       if ((rc = ensure(*w.p0, bytes))) return rc;
-      if (mode == SPLIT_TF32 && (rc = ensure(*w.p1, bytes))) return rc;
-      float *p0 = static_cast<float *>(w.p0->ptr), *p1 = mode == SPLIT_TF32 ? static_cast<float *>(w.p1->ptr) : nullptr;
-      rc = conv ? im2col_rows(c, o, mode, p0, p1, nullptr, nullptr, ld, nullptr, s, op)
-                : tf32_split(c, src, R, Cc, src_ld, p0, p1, ld, s, on_load, bt, cat);
+      if ((rc = ensure(*w.p1, bytes))) return rc;
+      rc = tf32_split(c, src, R, Cc, src_ld, static_cast<float *>(w.p0->ptr), static_cast<float *>(w.p1->ptr), ld, s, on_load, bt, cat);
     }
     if (rc) return rc;
   }
@@ -744,12 +757,9 @@ inline TcKind tc_kind_of_path(int path) {
 }
 inline SplitMode split_mode(TcKind k) { return k == TC_TF32X3 ? SPLIT_TF32 : k == TC_F16X3 ? SPLIT_F16X2 : SPLIT_NONE; }
 
-// a batched call: `batch` problems, operand X of problem b at X + b * X_stride (0: the batch shares it).  concat: the sum of
-// the problems' products into one C (C unused), i.e. one product over the operands concatenated along k (Operand::concat).
+// a batched launch: `batch` problems, C of problem b at C + b * C_stride
 struct BatchArgs {
-  int64_t batch;
-  int64_t A, B, C, auxA, auxB;
-  bool concat = false;
+  int64_t batch, C;
 };
 
 // launch the tensor-core kernel on prepared operands (c.mu held by the caller).  bat: a batched launch (tc_params.h; the maps
@@ -832,35 +842,30 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
   return prof.close();
 }
 
+// An operand -- with its op -- is the same in every problem of a batch: prepared once, read by every problem
+inline bool batch_shares(int64_t stride, const OperandOp *op, int64_t aux_stride) {
+  return stride == 0 && (!op || !op->aux || aux_stride == 0);
+}
+
 // SRC_ESZ: element size of the caller's operands (4: fp32 in any of the three tensor-core modes, 2: bf16)
 template <int SRC_ESZ, typename OutT>
-int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, const void *A, int64_t rsA,
-            int64_t csA, const void *B, int64_t rsB, int64_t csB, float beta, OutT *C, int64_t rsC,
-            int64_t csC, cudaStream_t s, const Epilogue &epi, cudaEvent_t b_ready = nullptr, const OperandOp *opA = nullptr,
-            const OperandOp *opB = nullptr, const BatchArgs *bat = nullptr, const ConvGeom *convB = nullptr) {
+int gemm_tc(Ctx &c, TcKind kind, const Operand &oa, const Operand &ob, float alpha, float beta, OutT *C, int64_t rsC, int64_t csC,
+            cudaStream_t s, const Epilogue &epi, cudaEvent_t b_ready = nullptr, const OperandOp *opA = nullptr,
+            const OperandOp *opB = nullptr, const BatchArgs *bat = nullptr) {
+  // oa / ob: A and B as built by run_f32 (bf16: single problems)
   // b_ready: B becomes valid only when this event has fired (the row-sharded driver: B is in flight on the communication
   // stream); everything that does not read B -- the preparation of A -- is queued before the wait.
   // opA / opB: operand ops applied while the operands are prepared (fp32 only)
-  // convB: B is an im2col source, the images at B (batched: bat->B floats apart; rsB, csB unused)
-  // bat->concat: one product of extent batch * K over the concatenated operands (one problem for the GEMM: rank-2 maps, one
-  // scale word per row of A and column of B)
-  const bool cat = bat && bat->concat;
-  const int64_t Kt = cat ? bat->batch * K : K;   // (the entry bounds batch * K by INT64_MAX)
+  // bat: a batched launch, every problem's operand in the same launches.  Concatenated operands (Operand::concat): one
+  // product of extent batch * K (one problem for the GEMM: rank-2 maps, one scale word per row of A and column of B).
+  const int64_t M = oa.mn, N = ob.mn, K = oa.k;
+  const bool cat = oa.concat;
+  const int64_t Kt = cat ? batch_of(oa).n * K : K;   // (the entry bounds batch * K by INT64_MAX)
   if (M > 0x7fffffffLL || N > 0x7fffffffLL || Kt > 0x7fffffffLL)
     return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: extents must fit in int32");
   std::lock_guard<std::mutex> lk(c.mu);  // workspace + descriptor construction are per context
   const SplitMode mode = split_mode(kind);
-  Operand oa{A, M, K, rsA, csA};
-  Operand ob{B, N, K, csB, rsB};
-  // bat: every problem's operand in the same launches (an operand -- op included -- that the batch shares: prepared once;
-  // concatenated: once per segment)
-  const bool a_shared = bat && !cat && bat->A == 0 && (!opA || !opA->aux || bat->auxA == 0);
-  const bool b_shared = bat && !cat && bat->B == 0 && (!opB || !opB->aux || bat->auxB == 0);
-  if (bat) {
-    oa.batch = a_shared ? 1 : bat->batch; oa.s_b = bat->A; oa.aux_sb = bat->auxA; oa.concat = cat;
-    ob.batch = b_shared ? 1 : bat->batch; ob.s_b = bat->B; ob.aux_sb = bat->auxB; ob.concat = cat;
-  }
-  ob.conv = convB;
+  const bool a_shared = bat && batch_shares(oa.s_b, opA, oa.aux_sb), b_shared = bat && batch_shares(ob.s_b, opB, ob.aux_sb);
   OperandMaps ma, mb;
   bool used_ws = false;
   // the previous call may still be reading the workspace on another stream
@@ -880,7 +885,7 @@ int gemm_tc(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, c
   const F16Scales f16{static_cast<const uint32_t *>(c.f16s.ptr), static_cast<const uint32_t *>(c.f16s.ptr) + f16_b_off};
   // (with profiling on, an event record sits between the last preparation kernel and the GEMM: no dependent launch then)
   rc = tc_run<OutT>(c, kind, M, N, Kt, alpha, ma, mb, beta, C, rsC, csC, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
-                    prep_launches > 0 && !c.profiling, cat ? nullptr : bat, a_shared, b_shared);
+                    prep_launches > 0 && !c.profiling, bat, a_shared, b_shared);
   if (rc) return rc;
   if (used_ws) CUDA_TRY(cudaEventRecord(c.ws_free, s));
   return LASER_B200_OK;
@@ -1035,25 +1040,69 @@ int resolve_auto(int64_t M, int64_t N, int64_t K, const Epilogue &epi, bool oper
   return mode < 0 ? kDefaultF32Mode : mode;
 }
 
-// Exact path with operand ops: each op'd operand is materialised once by the gather (compact [mn][k] workspace) and the
-// unchanged exact kernel multiplies that, so the path stays bit-identical to the CPU reference on the op'd operands.
-int gemm_simt_ops(Ctx &c, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
-                  const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC, cudaStream_t s,
-                  const Epilogue &epi, const OperandOp *opA, const OperandOp *opB) {
-  std::lock_guard<std::mutex> lk(c.mu);   // the gather buffers are workspace
-  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
+// the paths of the fp32 entries: PATH_AUTO, the exact kernel or a tensor-core mode
+int check_f32_path(int path) {
+  if (path == LASER_B200_PATH_AUTO || path == LASER_B200_PATH_SIMT || is_tc_mode(path)) return LASER_B200_OK;
+  return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+}
+
+// The exact path: each operand with an op, concatenated or an im2col source is written once into compact K-major rows of
+// the gather workspace (f32_rows, op applied), each other one is read in place; then one exact-kernel launch over the batch
+// (`batch` problems, C bsC apart), so the path stays bit-identical to the CPU reference on the operands as prepared.
+int simt_run(Ctx &c, const Operand &oa, const Operand &ob, float alpha, float beta, float *C, int64_t rsC, int64_t csC,
+             cudaStream_t s, const Epilogue &epi, const OperandOp *opA, const OperandOp *opB, int64_t batch, int64_t bsC) {
+  struct Rows {
+    const float *p;
+    int64_t s_mn, s_k, s_b;
+  };
+  const bool copy_a = opA || oa.concat || oa.conv, copy_b = opB || ob.concat || ob.conv;
+  std::unique_lock<std::mutex> lk(c.mu, std::defer_lock);   // the gather buffers are workspace
+  if (copy_a || copy_b) {
+    lk.lock();
+    CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
+  }
+  auto rows = [&](const Operand &o, const OperandOp *op, bool copy, Buffer &g, Rows *r) {
+    *r = Rows{static_cast<const float *>(o.ptr), o.s_mn, o.s_k, o.s_b};
+    if (!copy) return LASER_B200_OK;
+    const int rc = f32_rows(c, o, SPLIT_NONE, g, nullptr, s, op);
+    const int64_t ld = round_up(o.concat ? batch_of(o).n * o.k : o.k, 4);
+    *r = Rows{static_cast<const float *>(g.ptr), ld, 1, !o.concat && !batch_shares(o.s_b, op, o.aux_sb) ? o.mn * ld : 0};
+    return rc;
+  };
+  Rows a, b;
   int rc;
-  if (opA) {
-    if ((rc = gather<float>(c, Operand{A, M, K, rsA, csA}, c.gather[0], nullptr, s, opA))) return rc;
-    A = static_cast<const float *>(c.gather[0].ptr); rsA = round_up(K, 4); csA = 1;
-  }
-  if (opB) {
-    if ((rc = gather<float>(c, Operand{B, N, K, csB, rsB}, c.gather[1], nullptr, s, opB))) return rc;
-    B = static_cast<const float *>(c.gather[1].ptr); rsB = 1; csB = round_up(K, 4);
-  }
-  if ((rc = gemm_simt<float>(c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi))) return rc;
-  CUDA_TRY(cudaEventRecord(c.ws_free, s));
+  if ((rc = rows(oa, opA, copy_a, c.gather[0], &a))) return rc;
+  if ((rc = rows(ob, opB, copy_b, c.gather[1], &b))) return rc;
+  const int64_t K = oa.concat ? batch_of(oa).n * oa.k : oa.k;
+  if ((rc = gemm_simt<float>(c, oa.mn, ob.mn, K, alpha, a.p, a.s_mn, a.s_k, b.p, b.s_k, b.s_mn, beta, C, rsC, csC, s, epi, batch,
+                             a.s_b, b.s_b, bsC)))
+    return rc;
+  if (copy_a || copy_b) CUDA_TRY(cudaEventRecord(c.ws_free, s));
   return LASER_B200_OK;
+}
+
+// One fp32 product on a resolved path, the exact kernel or the tensor cores.  Its operands as [mn][k] (B: [n][k]):
+//   batch > 0: a batched call, operand X of problem b at X + b * bs->X and the aux of its op bs->auxX apart; an operand the
+//     batch shares, op included, is one problem, prepared once.  The problems' C bs->C apart.
+//   concat: the sum of the batch's products into one C, one product over the operands concatenated along k
+//     (Operand::concat; bs->C unused).
+//   convB: B is an im2col source, the images at B bs->B floats apart (rsB, csB unused).
+int run_f32(Ctx &c, int path, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA, const float *B,
+            int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC, cudaStream_t s, const Epilogue &epi,
+            const OperandOp *opA, const OperandOp *opB, int64_t batch = 0, const laser_b200_batch_strides *bs = nullptr,
+            bool concat = false, const ConvGeom *convB = nullptr, cudaEvent_t b_ready = nullptr) {
+  Operand oa{A, M, K, rsA, csA}, ob{B, N, K, csB, rsB};
+  if (batch > 0) {
+    oa.batch = !concat && batch_shares(bs->A, opA, bs->auxA) ? 1 : batch; oa.s_b = bs->A; oa.aux_sb = bs->auxA; oa.concat = concat;
+    ob.batch = !concat && batch_shares(bs->B, opB, bs->auxB) ? 1 : batch; ob.s_b = bs->B; ob.aux_sb = bs->auxB; ob.concat = concat;
+  }
+  ob.conv = convB;
+  const bool batched = batch > 0 && !concat;
+  if (path == LASER_B200_PATH_SIMT)
+    return simt_run(c, oa, ob, alpha, beta, C, rsC, csC, s, epi, opA, opB, batched ? batch : 1, batched ? bs->C : 0);
+  const BatchArgs bat{batch, batched ? bs->C : 0};
+  return gemm_tc<4, float>(c, tc_kind_of_path(path), oa, ob, alpha, beta, C, rsC, csC, s, epi, b_ready, opA, opB,
+                           batched ? &bat : nullptr);
 }
 
 // opA / opB: operand ops of the fused-prologue entry (nullptr: none)
@@ -1065,7 +1114,7 @@ int f32_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_
   if (rc == -1) return LASER_B200_OK;
   if (rc) return rc;
   const bool has_op = opA || opB;
-  if (has_op && path == -1) return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  if ((has_op || path != -1) && (rc = check_f32_path(path))) return rc;   // (-1: the GEMV, for calls without an op)
   Ctx *c;
   rc = get_ctx(&c);
   if (rc) return rc;
@@ -1097,24 +1146,15 @@ int f32_dev(int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_
       g_last_path = LASER_B200_PATH_SIMT;
       break;
     }
-    case LASER_B200_PATH_SIMT:
-      if (has_op) rc = gemm_simt_ops(*c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, opA, opB);
-      else rc = gemm_simt<float>(*c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi);
-      if (rc) return rc;
-      g_last_path = LASER_B200_PATH_SIMT;
-      break;
-    case LASER_B200_PATH_TF32X1:
-    case LASER_B200_PATH_TF32X3:
-    case LASER_B200_PATH_F16X3:
-      // F16X3 (default): two fp16 pieces of each operand scaled by a power of two per row of A / column of B (device-side
-      // abs-max), three passes, the epilogue undoes the scales.  TF32X3: hi/lo tf32 pieces, three passes.  TF32X1: one pass.
-      rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, b_ready,
-                             opA, opB);
+    default:
+      // SIMT: the exact kernel.  F16X3 (default): two fp16 pieces of each operand scaled by a power of two per row of A /
+      // column of B (device-side abs-max), three passes, the epilogue undoes the scales.  TF32X3: hi/lo tf32 pieces, three
+      // passes.  TF32X1: one pass.
+      rc = run_f32(*c, path, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, opA, opB, 0, nullptr, false,
+                   nullptr, b_ready);
       if (rc) return rc;
       g_last_path = path;
       break;
-    default:
-      return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
   }
   return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
@@ -1146,7 +1186,8 @@ int bf16_dev(int64_t M, int64_t N, int64_t K, float alpha, const uint16_t *A, in
   rc = get_ctx(&c);
   if (rc) return rc;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  rc = gemm_tc<2, uint16_t>(*c, TC_BF16, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, Epilogue());
+  rc = gemm_tc<2, uint16_t>(*c, TC_BF16, Operand{A, M, K, rsA, csA}, Operand{B, N, K, csB, rsB}, alpha, beta, C, rsC, csC, s,
+                            Epilogue());
   if (rc) return rc;
   g_last_path = LASER_B200_PATH_BF16;
   return finish(*c, static_cast<cudaStream_t>(stream), s);
@@ -1176,15 +1217,23 @@ int operand_op_of(const laser_b200_operand_op *in, bool is_b, OperandOp *op, con
   *out = op;
   return LASER_B200_OK;
 }
+// epilogue and operand ops of a fused GEMM entry, all checked before anything is launched (opA / opB: nullptr, or they point
+// into a / b -- a FusedArgs is used where it was decoded, never copied)
+struct FusedArgs {
+  Epilogue epi;
+  OperandOp a, b;
+  const OperandOp *opA = nullptr, *opB = nullptr;
+};
+int fused_args_of(const laser_b200_epilogue *epi, const laser_b200_operand_op *opA, const laser_b200_operand_op *opB, FusedArgs *f) {
+  int rc;
+  if ((rc = epilogue_of(epi, &f->epi))) return rc;
+  if ((rc = operand_op_of(opA, false, &f->a, &f->opA))) return rc;
+  return operand_op_of(opB, true, &f->b, &f->opB);
+}
 
 // ---------------------------------------------------------------------------------------
 //              batched fused product: the problems of a batch in one GEMM launch
 // ---------------------------------------------------------------------------------------
-// An operand -- with its op -- is the same in every problem: prepared once, read by every problem
-inline bool batch_shares(int64_t stride, const OperandOp *op, int64_t aux_stride) {
-  return stride == 0 && (!op || !op->aux || aux_stride == 0);
-}
-
 // workspace one problem of a batched call prepares on `path` (bytes, an upper bound): the pieces, gather copy and scale words
 // of each operand the problems do not share
 int64_t batch_ws_per_problem(int path, int64_t M, int64_t N, int64_t K, bool a_own, bool b_own, bool opA, bool opB) {
@@ -1198,70 +1247,39 @@ int64_t batch_ws_per_problem(int path, int64_t M, int64_t N, int64_t K, bool a_o
   return (a_own ? one(M, opA) : 0) + (b_own ? one(N, opB) : 0);
 }
 
-// problems [0, bat.batch) of a batched call on the resolved path: one preparation launch per step and operand, one GEMM launch
-int batched_run(Ctx &c, int path, const BatchArgs &bat, int64_t M, int64_t N, int64_t K, float alpha, const float *A,
-                int64_t rsA, int64_t csA, const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC,
-                int64_t csC, cudaStream_t s, const Epilogue &epi, const OperandOp *opA, const OperandOp *opB) {
-  if (path != LASER_B200_PATH_SIMT)
-    return gemm_tc<4, float>(c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, nullptr,
-                             opA, opB, &bat);
-  int64_t bsA = bat.A, bsB = bat.B;
-  if (!opA && !opB)
-    return gemm_simt<float>(c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, bat.batch, bsA, bsB, bat.C);
-  // exact path with ops: the batched gather materialises every problem's op'd operand (gemm_simt_ops, batched)
-  std::lock_guard<std::mutex> lk(c.mu);
-  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
-  int rc;
-  if (opA) {
-    const bool shared = batch_shares(bat.A, opA, bat.auxA);
-    if ((rc = gather<float>(c, Operand{A, M, K, rsA, csA, shared ? 1 : bat.batch, bat.A, bat.auxA}, c.gather[0], nullptr, s, opA)))
-      return rc;
-    A = static_cast<const float *>(c.gather[0].ptr); rsA = round_up(K, 4); csA = 1; bsA = shared ? 0 : M * rsA;
-  }
-  if (opB) {
-    const bool shared = batch_shares(bat.B, opB, bat.auxB);
-    if ((rc = gather<float>(c, Operand{B, N, K, csB, rsB, shared ? 1 : bat.batch, bat.B, bat.auxB}, c.gather[1], nullptr, s, opB)))
-      return rc;
-    B = static_cast<const float *>(c.gather[1].ptr); rsB = 1; csB = round_up(K, 4); bsB = shared ? 0 : N * csB;
-  }
-  if ((rc = gemm_simt<float>(c, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, bat.batch, bsA, bsB, bat.C)))
-    return rc;
-  CUDA_TRY(cudaEventRecord(c.ws_free, s));
-  return LASER_B200_OK;
-}
-
+// convB: B is an im2col source (a convolution, run_f32): even one image takes the batched launch
 int batched_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
                       const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
                       const laser_b200_batch_strides *bs, const OperandOp *opA, const OperandOp *opB, const Epilogue &epi,
-                      int path, void *stream) {
+                      int path, void *stream, const ConvGeom *convB = nullptr) {
   if (batch < 0) return set_error(LASER_B200_EINVAL, "negative batch %lld", (long long)batch);
   if (batch > 0 && !bs) return set_error(LASER_B200_EINVAL, "batchStrides is NULL");
   if (batch > 1 && bs->C == 0) return set_error(LASER_B200_EINVAL, "batchStrides->C is 0: the problems' outputs would overlap");
-  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
-    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
-  int rc = check_args(M, N, K, A, B, C);
+  int rc;
+  if ((rc = check_f32_path(path))) return rc;
+  rc = check_args(M, N, K, A, B, C);
   if (rc == -1 || batch == 0) return LASER_B200_OK;
   if (rc) return rc;
-  if (batch == 1) return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, epi, nullptr, opA, opB);
+  if (batch == 1 && !convB)
+    return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, epi, nullptr, opA, opB);
   Ctx *c;
   if ((rc = get_ctx(&c))) return rc;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
   if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, K, epi, /*operand_op=*/true);
   // chunks of whole problems: the prepared workspace stays under the cap, and the launch's tile counts -- batch x tiles x
-  // up to 16 K-splits -- fit in int32
+  // up to 16 K-splits -- fit in int32 (an im2col source counts as an op'd B: the exact path writes its rows)
   const int64_t per = batch_ws_per_problem(path, M, N, K, !batch_shares(bs->A, opA, bs->auxA), !batch_shares(bs->B, opB, bs->auxB),
-                                           opA != nullptr, opB != nullptr);
+                                           opA != nullptr, opB != nullptr || convB);
   int64_t chunk = per > 0 ? c->batch_ws_bytes / per : batch;
   const int64_t tiles = ((M + TC_BLOCK_M - 1) / TC_BLOCK_M) * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N);
   if (chunk > 0x7fffffffLL / (16 * tiles)) chunk = 0x7fffffffLL / (16 * tiles);
   if (chunk < 1) chunk = 1;
   for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
-    const BatchArgs bat{batch - b0 < chunk ? batch - b0 : chunk, bs->A, bs->B, bs->C, bs->auxA, bs->auxB};
     OperandOp ca, cb;
     if (opA) { ca = *opA; if (ca.aux) ca.aux += b0 * bs->auxA; }
     if (opB) { cb = *opB; if (cb.aux) cb.aux += b0 * bs->auxB; }
-    if ((rc = batched_run(*c, path, bat, M, N, K, alpha, A + b0 * bs->A, rsA, csA, B + b0 * bs->B, rsB, csB, beta, C + b0 * bs->C, rsC,
-                          csC, s, epi, opA ? &ca : nullptr, opB ? &cb : nullptr)))
+    if ((rc = run_f32(*c, path, M, N, K, alpha, A + b0 * bs->A, rsA, csA, B + b0 * bs->B, rsB, csB, beta, C + b0 * bs->C, rsC, csC, s,
+                      epi, opA ? &ca : nullptr, opB ? &cb : nullptr, batch - b0 < chunk ? batch - b0 : chunk, bs, false, convB)))
       return rc;
   }
   g_last_path = path;
@@ -1272,77 +1290,41 @@ int batched_fused_entry(int64_t batch, int64_t M, int64_t N, int64_t K, float al
                         const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
                         const laser_b200_batch_strides *bs, const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
                         const laser_b200_epilogue *epi, int path, void *stream) {
-  Epilogue e;
-  OperandOp oa, ob;
-  const OperandOp *pa, *pb;
-  int rc;
-  if ((rc = epilogue_of(epi, &e))) return rc;
-  if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
-  if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
-  return batched_fused_dev(batch, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, bs, pa, pb, e, path, stream);
+  FusedArgs f;
+  const int rc = fused_args_of(epi, opA, opB, &f);
+  if (rc) return rc;
+  return batched_fused_dev(batch, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, bs, f.opA, f.opB, f.epi, path, stream);
 }
 
 // ---------------------------------------------------------------------------------------
 //   batch-reduced fused product: the sum of a batch's products, one product over the operands concatenated along k
 // ---------------------------------------------------------------------------------------
-// Exact path: the gather writes each operand concatenated (op applied) into compact [mn][batch * K] rows, and the unchanged
-// exact kernel multiplies those, so the path stays bit-identical to the CPU reference over the concatenation.  convB: B is a
-// concatenated im2col source (the images at B, bat.B floats apart), its plain tap rows written by im2col_rows.
-int batch_reduce_simt(Ctx &c, const BatchArgs &bat, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA,
-                      int64_t csA, const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
-                      cudaStream_t s, const Epilogue &epi, const OperandOp *opA, const OperandOp *opB,
-                      const ConvGeom *convB = nullptr) {
-  const int64_t Kt = bat.batch * K, ld = round_up(Kt, 4);
-  Operand oa{A, M, K, rsA, csA, bat.batch, bat.A, bat.auxA}, ob{B, N, K, csB, rsB, bat.batch, bat.B, bat.auxB};
-  oa.concat = ob.concat = true;
-  ob.conv = convB;
-  std::lock_guard<std::mutex> lk(c.mu);   // the gather buffers are workspace
-  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
-  int rc;
-  if ((rc = gather<float>(c, oa, c.gather[0], nullptr, s, opA))) return rc;
-  if (convB) {
-    if ((rc = ensure(c.gather[1], static_cast<size_t>(N) * ld * sizeof(float)))) return rc;
-    rc = im2col_rows(c, ob, SPLIT_NONE, static_cast<float *>(c.gather[1].ptr), nullptr, nullptr, nullptr, ld, nullptr, s);
-  } else {
-    rc = gather<float>(c, ob, c.gather[1], nullptr, s, opB);
-  }
-  if (rc) return rc;
-  if ((rc = gemm_simt<float>(c, M, N, Kt, alpha, static_cast<const float *>(c.gather[0].ptr), ld, 1,
-                             static_cast<const float *>(c.gather[1].ptr), 1, ld, beta, C, rsC, csC, s, epi)))
-    return rc;
-  CUDA_TRY(cudaEventRecord(c.ws_free, s));
-  return LASER_B200_OK;
-}
-
 // laser_b200_gemm_strided_batch_reduce_f32_fused_dev: C <- act(alpha * sum_b opA(A_b) * opB(B_b) + beta * C + bias), the fused
 // call over A^ = [opA(A_0) | .. | opA(A_{n-1})] (M x nK) and B^ = [opB(B_0); ..; opB(B_{n-1})] (nK x N).  One chunk always:
-// chunking a sum would round C between chunks and apply the activation too early.
+// chunking a sum would round C between chunks and apply the activation too early.  convB: B is a concatenated im2col source
+// (a convolution's filter gradient, run_f32): even one image takes the concatenated preparation.
 int batch_reduce_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
                      const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
                      const laser_b200_batch_strides *bs, const OperandOp *opA, const OperandOp *opB, const Epilogue &epi, int path,
-                     void *stream) {
+                     void *stream, const ConvGeom *convB = nullptr) {
   if (batch < 0) return set_error(LASER_B200_EINVAL, "negative batch %lld", (long long)batch);
   if (batch > 0 && !bs) return set_error(LASER_B200_EINVAL, "batchStrides is NULL");
   if (batch > 0 && bs->C != 0)
     return set_error(LASER_B200_EINVAL, "batchStrides->C is %lld: the batch sums into one C", (long long)bs->C);
-  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
-    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
-  int rc = check_args(M, N, K, A, B, C);
+  int rc;
+  if ((rc = check_f32_path(path))) return rc;
+  rc = check_args(M, N, K, A, B, C);
   if (rc == -1 || batch == 0) return LASER_B200_OK;
   if (rc) return rc;
-  if (batch == 1) return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, epi, nullptr, opA, opB);
+  if (batch == 1 && !convB)
+    return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, epi, nullptr, opA, opB);
   if (K > INT64_MAX / batch) return set_error(LASER_B200_EUNSUPPORTED, "batch * K overflows int64");
   Ctx *c;
   if ((rc = get_ctx(&c))) return rc;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
   if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, batch * K, epi, /*operand_op=*/true);
-  const BatchArgs bat{batch, bs->A, bs->B, 0, bs->auxA, bs->auxB, true};
-  if (path == LASER_B200_PATH_SIMT)
-    rc = batch_reduce_simt(*c, bat, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, opA, opB);
-  else
-    rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, nullptr,
-                           opA, opB, &bat);
-  if (rc) return rc;
+  if ((rc = run_f32(*c, path, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, s, epi, opA, opB, batch, bs, true, convB)))
+    return rc;
   g_last_path = path;
   return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
@@ -1350,68 +1332,22 @@ int batch_reduce_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha
 // ---------------------------------------------------------------------------------------
 //     fused convolution: im2col folded into the preparation of B, the images of a chunk in one GEMM launch
 // ---------------------------------------------------------------------------------------
-// Exact path, `images` images: their windows as plain K-major rows in the gather workspace (opB applied), one batched
-// exact-kernel launch with A = [Cout][K] rows lda apart
-int conv2d_simt(Ctx &c, const ConvGeom &g, int64_t images, float alpha, const float *A, int64_t lda, const float *input, float beta,
-                float *output, cudaStream_t s, const Epilogue &epi, const OperandOp *opB) {
-  const int64_t M = g.Cout, K = g.K(), N = g.outHW(), ld = round_up(K, 4);
-  std::lock_guard<std::mutex> lk(c.mu);   // the gather buffer is workspace
-  CUDA_TRY(cudaStreamWaitEvent(s, c.ws_free, 0));
-  int rc;
-  if ((rc = ensure(c.gather[1], static_cast<size_t>(images * N) * ld * sizeof(float)))) return rc;
-  Operand o{input, N, K, 0, 0, images, g.C * g.H * g.W};
-  o.conv = &g;
-  float *rows = static_cast<float *>(c.gather[1].ptr);
-  if ((rc = im2col_rows(c, o, SPLIT_NONE, rows, nullptr, nullptr, nullptr, ld, nullptr, s, opB))) return rc;
-  if ((rc = gemm_simt<float>(c, M, N, K, alpha, A, lda, 1, rows, 1, ld, beta, output, N, 1, s, epi, images, 0, N * ld, M * N)))
-    return rc;
-  CUDA_TRY(cudaEventRecord(c.ws_free, s));
-  return LASER_B200_OK;
-}
-
 // The product of both fused convolution entries, image by image: output_n = epi(alpha * A * B_n + beta * output_n), A [Cout][K]
 // (rsA, csA; K-major with 16-byte rows unless the kernel is 1 x 1), shared by the images; B_n image n of `input` as an im2col
-// source of geometry g (dilated: ConvGeom::dH, dW), opB applied to its values (aux dense like `input`).  Chunks of whole
-// images under LASER_B200_BATCH_WS_MB: the images do not sum into each other.
+// source of geometry g (dilated: ConvGeom::dH, dW), opB applied to its values (aux dense like `input`).  The batched fused
+// product over the images, in its chunks of whole images under LASER_B200_BATCH_WS_MB: the images do not sum into each other.
 int conv_windows_dev(const ConvGeom &g, float alpha, const float *A, int64_t rsA, int64_t csA, const float *input, float beta,
                      float *output, const OperandOp *opB, const Epilogue &epi, int path, void *stream) {
-  int rc;
   const int64_t M = g.Cout, K = g.K(), N = g.outHW(), image = g.C * g.H * g.W;
   // PATH_AUTO decides as conv2d_im2col_f32_dev does: the exact kernel for a batch of short M or K (batched_f32_dev), else
   // resolve_auto with this call's epilogue (never the GEMV: N is a pixel count and the batch needs one launch)
   if (path == LASER_B200_PATH_AUTO)
     path = (g.B > 1 && (M < 64 || K < 64)) ? LASER_B200_PATH_SIMT : resolve_auto(M, N, K, epi, /*operand_op=*/true);
-  if (g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0 && g.dH == 1 && g.dW == 1) {
-    // the image already is the [C][H*W] matrix
-    const laser_b200_batch_strides bs{0, image, M * N, 0, image};
-    return batched_fused_dev(g.B, M, N, K, alpha, A, rsA, csA, input, N, 1, beta, output, N, 1, &bs, nullptr, opB, epi, path, stream);
-  }
-  Ctx *c;
-  if ((rc = get_ctx(&c))) return rc;
-  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  // chunks of whole images, as batched_fused_dev makes them (the exact path's rows count as an op'd B)
-  const int64_t per = batch_ws_per_problem(path, M, N, K, false, true, false, true);
-  int64_t chunk = c->batch_ws_bytes / per;
-  const int64_t tiles = ((M + TC_BLOCK_M - 1) / TC_BLOCK_M) * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N);
-  if (chunk > 0x7fffffffLL / (16 * tiles)) chunk = 0x7fffffffLL / (16 * tiles);
-  if (chunk < 1) chunk = 1;
-  for (int64_t n0 = 0; n0 < g.B; n0 += chunk) {
-    const int64_t cnt = g.B - n0 < chunk ? g.B - n0 : chunk;
-    const float *in = input + n0 * image;
-    float *out = output + n0 * M * N;
-    OperandOp ob;
-    if (opB) { ob = *opB; if (ob.aux) ob.aux += n0 * image; }
-    if (path == LASER_B200_PATH_SIMT) {
-      rc = conv2d_simt(*c, g, cnt, alpha, A, rsA, in, beta, out, s, epi, opB ? &ob : nullptr);
-    } else {
-      const BatchArgs bat{cnt, 0, image, M * N, 0, image};
-      rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, K, alpha, A, rsA, csA, in, 0, 0, beta, out, N, 1, s, epi, nullptr, nullptr,
-                             opB ? &ob : nullptr, &bat, &g);
-    }
-    if (rc) return rc;
-  }
-  g_last_path = path;
-  return finish(*c, static_cast<cudaStream_t>(stream), s);
+  // a 1 x 1 kernel with unit strides, no padding and no dilation: the image already is B_n, the [C][H*W] matrix
+  const bool in_place = g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0 && g.dH == 1 && g.dW == 1;
+  const laser_b200_batch_strides bs{0, image, M * N, 0, image};
+  return batched_fused_dev(g.B, M, N, K, alpha, A, rsA, csA, input, N, 1, beta, output, N, 1, &bs, nullptr, opB, epi, path, stream,
+                           in_place ? nullptr : &g);
 }
 
 // laser_b200_conv2d_f32_fused_dev (capi_layers.inc checks the geometry): output_n = act(F * im2col(input_n) + bias) for every
@@ -1421,8 +1357,7 @@ int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const
   Epilogue epi;
   int rc;
   if ((rc = epilogue_of(epi_in, &epi))) return rc;
-  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
-    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  if ((rc = check_f32_path(path))) return rc;
   if (g.B == 0) return LASER_B200_OK;
   if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
   return conv_windows_dev(g, 1.0f, kernel, g.K(), 1, input, 0.0f, output, nullptr, epi, path, stream);
@@ -1441,11 +1376,10 @@ int launch_copy(Ctx &c, void *dst, const void *src, const CopyParams &p, cudaStr
 // Im2colGradSrc).  M = C, N = H * W, K' = Cout * kH * kW; conv_windows_dev runs it as it runs the forward call.
 int conv2d_input_grad_dev(float *grad_input, const ConvGeom &g, const float *grad_output, const float *kernel, float alpha, float beta,
                           const laser_b200_operand_op *op_in, int path, void *stream) {
-  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
-    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  int rc;
+  if ((rc = check_f32_path(path))) return rc;
   OperandOp op;
   const OperandOp *opB;
-  int rc;
   if ((rc = operand_op_of(op_in, true, &op, &opB))) return rc;
   const int64_t P = g.outHW(), khw = g.kH * g.kW;
   // (B seen as [mn = pixel][k = channel]: a dense NCHW aux has aux_sr = 1, aux_sc = outH * outW)
@@ -1492,11 +1426,10 @@ int conv2d_input_grad_dev(float *grad_input, const ConvGeom &g, const float *gra
 // batch_reduce_dev: chunks would round dW between them.
 int conv2d_filter_grad_dev(float *grad_kernel, const float *input, const ConvGeom &g, const float *grad_output, float alpha,
                            float beta, const laser_b200_operand_op *op_in, int path, void *stream) {
-  if (path != LASER_B200_PATH_AUTO && path != LASER_B200_PATH_SIMT && !is_tc_mode(path))
-    return set_error(LASER_B200_EINVAL, "unknown path %d for float32", path);
+  int rc;
+  if ((rc = check_f32_path(path))) return rc;
   OperandOp op;
   const OperandOp *opA;
-  int rc;
   if ((rc = operand_op_of(op_in, false, &op, &opA))) return rc;
   const int64_t M = g.Cout, N = g.K(), P = g.outHW(), image = g.C * g.H * g.W;
   if (opA && opA->aux && (opA->aux_sr != P || opA->aux_sc != 1))
@@ -1505,27 +1438,11 @@ int conv2d_filter_grad_dev(float *grad_kernel, const float *input, const ConvGeo
   if (g.B == 0) return LASER_B200_OK;
   if (!grad_kernel || !input || !grad_output) return set_error(LASER_B200_EINVAL, "null pointer");
   // B of a 1 x 1 kernel with unit strides and no padding is the images read in place: B_n[p][c] = input_n[c][p]
-  if (g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0) {
-    const laser_b200_batch_strides bs{M * P, image, 0, M * P, 0};
-    return batch_reduce_dev(g.B, M, N, P, alpha, grad_output, P, 1, input, 1, P, beta, grad_kernel, N, 1, &bs, opA, nullptr,
-                            Epilogue(), path, stream);
-  }
-  if (P > INT64_MAX / g.B) return set_error(LASER_B200_EUNSUPPORTED, "images * outH * outW overflows int64");
-  Ctx *c;
-  if ((rc = get_ctx(&c))) return rc;
-  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  // PATH_AUTO decides as batch_reduce_dev does over K' = images * P (with an operand op: B is prepared, never the GEMV)
-  if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, g.B * P, Epilogue(), /*operand_op=*/true);
-  const BatchArgs bat{g.B, M * P, image, 0, M * P, 0, true};
-  if (path == LASER_B200_PATH_SIMT)
-    rc = batch_reduce_simt(*c, bat, M, N, P, alpha, grad_output, P, 1, input, 0, 0, beta, grad_kernel, N, 1, s, Epilogue(), opA,
-                           nullptr, &g);
-  else
-    rc = gemm_tc<4, float>(*c, tc_kind_of_path(path), M, N, P, alpha, grad_output, P, 1, input, 0, 0, beta, grad_kernel, N, 1, s,
-                           Epilogue(), nullptr, opA, nullptr, &bat, &g);
-  if (rc) return rc;
-  g_last_path = path;
-  return finish(*c, static_cast<cudaStream_t>(stream), s);
+  const bool in_place = g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0;
+  if (!in_place && P > INT64_MAX / g.B) return set_error(LASER_B200_EUNSUPPORTED, "images * outH * outW overflows int64");
+  const laser_b200_batch_strides bs{M * P, image, 0, M * P, 0};
+  return batch_reduce_dev(g.B, M, N, P, alpha, grad_output, P, 1, input, 1, P, beta, grad_kernel, N, 1, &bs, opA, nullptr, Epilogue(),
+                          path, stream, in_place ? nullptr : &g);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1826,28 +1743,21 @@ int laser_b200_gemm_strided_f32_fused_dev(int64_t M, int64_t N, int64_t K, float
                                           int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
                                           const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
                                           const laser_b200_epilogue *epi, int path, void *stream) {
-  Epilogue e;
-  OperandOp oa, ob;
-  const OperandOp *pa, *pb;
-  int rc;
-  if ((rc = epilogue_of(epi, &e))) return rc;
-  if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
-  if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
-  return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, e, nullptr, pa, pb);
+  FusedArgs f;
+  const int rc = fused_args_of(epi, opA, opB, &f);
+  if (rc) return rc;
+  return f32_dev(M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, path, stream, f.epi, nullptr, f.opA, f.opB);
 }
 int laser_b200_gemm_strided_batch_reduce_f32_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A,
                                                        int64_t rsA, int64_t csA, const float *B, int64_t rsB, int64_t csB, float beta,
                                                        float *C, int64_t rsC, int64_t csC, const laser_b200_batch_strides *batchStrides,
                                                        const laser_b200_operand_op *opA, const laser_b200_operand_op *opB,
                                                        const laser_b200_epilogue *epi, int path, void *stream) {
-  Epilogue e;
-  OperandOp oa, ob;
-  const OperandOp *pa, *pb;
-  int rc;
-  if ((rc = epilogue_of(epi, &e))) return rc;
-  if ((rc = operand_op_of(opA, false, &oa, &pa))) return rc;
-  if ((rc = operand_op_of(opB, true, &ob, &pb))) return rc;
-  return batch_reduce_dev(batch, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, batchStrides, pa, pb, e, path, stream);
+  FusedArgs f;
+  const int rc = fused_args_of(epi, opA, opB, &f);
+  if (rc) return rc;
+  return batch_reduce_dev(batch, M, N, K, alpha, A, rsA, csA, B, rsB, csB, beta, C, rsC, csC, batchStrides, f.opA, f.opB, f.epi, path,
+                          stream);
 }
 int laser_b200_gemm_strided_f64_dev(int64_t M, int64_t N, int64_t K, double alpha, const double *A,
                                     int64_t rsA, int64_t csA, const double *B, int64_t rsB,
