@@ -453,6 +453,28 @@ int laser_b200_conv2d_im2col_f32_dev(float *output, const float *input, const in
 int laser_b200_conv2d_f32_fused_dev(float *output, const float *input, const int64_t ishape[4],
                                     const float *kernel, const int64_t kshape[4], const int64_t padding[2],
                                     const int64_t strides[2], const laser_b200_epilogue *epi, int path, void *stream);
+/* Channels-last fused convolution (conv2d_mec's NHWC layout and [kH][kW][C_in][C_out] filters, benchmarks/convolution/
+ * conv2d_mec.nim, with padding): for every image n,
+ *   output_n <- act(conv(input_n, kernel) + bias)
+ * with ishape = (n, c, h, w) and kshape = (c_out, c_in, kH, kW) in the reference's tuple order, and the checks and output
+ * shape of conv2d_out_shape.  input is dense NHWC [n][h][w][c]; output is dense NHWC [n][outH][outW][c_out] and is fully
+ * overwritten (alpha 1, beta 0).  kernel is the filter matrix Wmat[(kh * kW + kw) * c_in + ci][co], read with the element
+ * strides kernelStrides = (over its rows, over output channels): {c_out, 1} for kernel_to_hwcc's [kH][kW][C_in][C_out],
+ * {1, kH * kW * c_in} for torch's channels_last weight [c_out][kH][kW][c_in]; any other strides work too.
+ *   The product of the images is ONE GEMM, output[n * P + p][co] = sum_k rows[n * P + p][k] * Wmat[k][co] (P = outH * outW),
+ *   whose A -- the im2col matrix, one row per output pixel -- is prepared straight from the images (16-byte loads along the
+ *   channels when c % 4 == 0 and input is 16-byte aligned).  1 x 1 kernels with unit strides and no padding read input in
+ *   place as the [n * h * w][c] matrix.  No workspace argument; chunks of whole images under LASER_B200_BATCH_WS_MB.
+ *   epi: bias_per_row = 1 is one bias per output channel (a bias with bias_per_row = 0 is EINVAL); NULL epi = no bias, no
+ *   activation.  path: as for the float32 GEMM; PATH_AUTO takes the path conv2d_f32_fused_dev takes for the same geometry.
+ *   n = 0: LASER_B200_OK, nothing launched, output untouched.  n * outH * outW must fit in int32 on the tensor-core paths
+ *   (LASER_B200_EUNSUPPORTED otherwise).
+ *   LASER_B200_EINVAL, before anything is launched: geometry errors, kshape[1] != c_in, kernelStrides NULL, an unknown path
+ *   or activation, the bias rule above, a NULL pointer. */
+int laser_b200_conv2d_nhwc_f32_fused_dev(float *output, const float *input, const int64_t ishape[4],
+                                         const float *kernel, const int64_t kshape[4], const int64_t kernelStrides[2],
+                                         const int64_t padding[2], const int64_t strides[2],
+                                         const laser_b200_epilogue *epi, int path, void *stream);
 /* Filter gradient of the fused convolution (derivatives applied while an operand is prepared for a backward product, and the
  * im2col prepacker, of the reference's fusion roadmap, README.md:244-245 and :251; the reference has no backward convolution):
  *   grad_kernel <- alpha * sum_n op(grad_output_n) * im2col(input_n)^T + beta * grad_kernel

@@ -583,26 +583,36 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
 // every image end to end (split.cuh: im2col_tap_rows_kernel), F16X2 after an abs-max pass over the same tiles.
 // A dilated source (ConvGeom::dH, dW) or an op: the transposed source of the input gradient, the rows kernel's DIL / HAS_OP
 // instantiations (op applied to the values read, its aux dense like the images; not with `concat`).
+// A channels-last source (ConvGeom::nhwc): the windows of NHWC images in (kh, kw, c) order, the rows kernel's NHWC
+// instantiations; one problem, mn = images * outH * outW rows.
 int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst_lo, uint16_t *hb, uint16_t *lb, int64_t ld,
                 uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
   const Im2colSrc q = im2col_src(*o.conv);
-  const int64_t images = batch_of(o).n, rows = images * o.mn;
+  const Batch bt = batch_of(o);
+  // the images of the launch: a batch of problems of outHW rows each (the NCHW sources), or one problem whose mn rows are the
+  // pixels of every image (the channels-last source, A of the NHWC forward call)
+  const int64_t images = o.concat ? bt.n : bt.n * (o.mn / q.outHW), rows = bt.n * o.mn;
   const int64_t tiles = o.mn * ((ld + TAP_SEG - 1) / TAP_SEG);
   const float *in = static_cast<const float *>(o.ptr);
   const bool dil = o.conv->dH != 1 || o.conv->dW != 1;
   if (o.concat && (dil || op)) return set_error(LASER_B200_ECUDA, "internal: a concatenated im2col source has no dilation or op");
+  if (o.conv->nhwc && (o.concat || dil || op))
+    return set_error(LASER_B200_ECUDA, "internal: a channels-last im2col source is not concatenated, dilated or op'd");
   auto launch = [&](auto m, auto absmax) {
     constexpr int MODE = decltype(m)::value, PER_SM = MODE == IM2COL_F16X2 ? 3 : 4;   // the kernel's launch bounds
     auto rows_kernel = [&](auto d, auto has_op, const auto &src) {
       constexpr bool DIL = decltype(d)::value, HAS_OP = decltype(has_op)::value;
+      constexpr bool NHWC = std::is_same<typename std::decay<decltype(src)>::type, Im2colNhwcSrc>::value;
       if (ld <= 4 * 32 * F16ROWS_MAXV)
-        im2col_rows_kernel<MODE, 32, DIL, HAS_OP><<<grid_for(c, (rows + 7) / 8, PER_SM), 256, 0, s>>>(in, src, images, dst, dst_lo, hb,
-                                                                                                   lb, ld, words);
+        im2col_rows_kernel<MODE, 32, DIL, HAS_OP, NHWC><<<grid_for(c, (rows + 7) / 8, PER_SM), 256, 0, s>>>(in, src, images, dst,
+                                                                                                         dst_lo, hb, lb, ld, words);
       else
-        im2col_rows_kernel<MODE, 256, DIL, HAS_OP><<<grid_for(c, rows, PER_SM), 256, 0, s>>>(in, src, images, dst, dst_lo, hb, lb, ld,
-                                                                                          words);
+        im2col_rows_kernel<MODE, 256, DIL, HAS_OP, NHWC><<<grid_for(c, rows, PER_SM), 256, 0, s>>>(in, src, images, dst, dst_lo, hb,
+                                                                                                lb, ld, words);
     };
-    if (o.concat) {
+    if (o.conv->nhwc) {
+      rows_kernel(std::false_type(), std::false_type(), im2col_nhwc_src(*o.conv, in));
+    } else if (o.concat) {
       im2col_tap_rows_kernel<MODE, decltype(absmax)::value><<<grid_for(c, tiles, 8), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb,
                                                                                                  ld, words);
     } else if (dil || op) {
@@ -1087,15 +1097,18 @@ int simt_run(Ctx &c, const Operand &oa, const Operand &ob, float alpha, float be
 //   concat: the sum of the batch's products into one C, one product over the operands concatenated along k
 //     (Operand::concat; bs->C unused).
 //   convB: B is an im2col source, the images at B bs->B floats apart (rsB, csB unused).
+//   convA: A is a channels-last im2col source (ConvGeom::nhwc), M = images * outH * outW rows of the images at A (rsA, csA
+//     unused; a single problem).
 int run_f32(Ctx &c, int path, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA, const float *B,
             int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC, cudaStream_t s, const Epilogue &epi,
             const OperandOp *opA, const OperandOp *opB, int64_t batch = 0, const laser_b200_batch_strides *bs = nullptr,
-            bool concat = false, const ConvGeom *convB = nullptr, cudaEvent_t b_ready = nullptr) {
+            bool concat = false, const ConvGeom *convB = nullptr, cudaEvent_t b_ready = nullptr, const ConvGeom *convA = nullptr) {
   Operand oa{A, M, K, rsA, csA}, ob{B, N, K, csB, rsB};
   if (batch > 0) {
     oa.batch = !concat && batch_shares(bs->A, opA, bs->auxA) ? 1 : batch; oa.s_b = bs->A; oa.aux_sb = bs->auxA; oa.concat = concat;
     ob.batch = !concat && batch_shares(bs->B, opB, bs->auxB) ? 1 : batch; ob.s_b = bs->B; ob.aux_sb = bs->auxB; ob.concat = concat;
   }
+  oa.conv = convA;
   ob.conv = convB;
   const bool batched = batch > 0 && !concat;
   if (path == LASER_B200_PATH_SIMT)
@@ -1336,13 +1349,18 @@ int batch_reduce_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha
 // (rsA, csA; K-major with 16-byte rows unless the kernel is 1 x 1), shared by the images; B_n image n of `input` as an im2col
 // source of geometry g (dilated: ConvGeom::dH, dW), opB applied to its values (aux dense like `input`).  The batched fused
 // product over the images, in its chunks of whole images under LASER_B200_BATCH_WS_MB: the images do not sum into each other.
+// PATH_AUTO of a convolution of geometry g, in either layout: as conv2d_im2col_f32_dev decides, the exact kernel for a batch of
+// short M = c_out or K (batched_f32_dev), else resolve_auto over one NCHW image's product with this call's epilogue (never
+// the GEMV: N is a pixel count and the batch needs one launch)
+int conv_auto_path(const ConvGeom &g, const Epilogue &epi) {
+  const int64_t M = g.Cout, K = g.K();
+  return (g.B > 1 && (M < 64 || K < 64)) ? LASER_B200_PATH_SIMT : resolve_auto(M, g.outHW(), K, epi, /*operand_op=*/true);
+}
+
 int conv_windows_dev(const ConvGeom &g, float alpha, const float *A, int64_t rsA, int64_t csA, const float *input, float beta,
                      float *output, const OperandOp *opB, const Epilogue &epi, int path, void *stream) {
   const int64_t M = g.Cout, K = g.K(), N = g.outHW(), image = g.C * g.H * g.W;
-  // PATH_AUTO decides as conv2d_im2col_f32_dev does: the exact kernel for a batch of short M or K (batched_f32_dev), else
-  // resolve_auto with this call's epilogue (never the GEMV: N is a pixel count and the batch needs one launch)
-  if (path == LASER_B200_PATH_AUTO)
-    path = (g.B > 1 && (M < 64 || K < 64)) ? LASER_B200_PATH_SIMT : resolve_auto(M, N, K, epi, /*operand_op=*/true);
+  if (path == LASER_B200_PATH_AUTO) path = conv_auto_path(g, epi);
   // a 1 x 1 kernel with unit strides, no padding and no dilation: the image already is B_n, the [C][H*W] matrix
   const bool in_place = g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0 && g.dH == 1 && g.dW == 1;
   const laser_b200_batch_strides bs{0, image, M * N, 0, image};
@@ -1361,6 +1379,52 @@ int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const
   if (g.B == 0) return LASER_B200_OK;
   if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
   return conv_windows_dev(g, 1.0f, kernel, g.K(), 1, input, 0.0f, output, nullptr, epi, path, stream);
+}
+
+// laser_b200_conv2d_nhwc_f32_fused_dev (capi_layers.inc checks the geometry): NHWC images, one product for the images of a chunk,
+//   output[n * P + p][co] = act(sum_k rows[n * P + p][k] * Wmat[k][co] + bias[co]),  P = outH * outW
+// A = the images as a channels-last im2col source (one row per output pixel, K-major), B = the filter matrix [K][c_out] read
+// with its strides (kernelStrides[0] over k, [1] over co), C = the NHWC output, the bias one per column.  1 x 1 kernels with unit strides
+// and no padding: A is the images read in place as [n * H * W][C].  Chunks of whole images under LASER_B200_BATCH_WS_MB, the
+// tile count of each in int32, one preparation and one GEMM launch sequence each.
+int conv2d_nhwc_fused_dev(float *output, const float *input, const ConvGeom &g, const float *kernel, const int64_t kernelStrides[2],
+                          const laser_b200_epilogue *epi_in, int path, void *stream) {
+  Epilogue epi;
+  int rc;
+  if ((rc = epilogue_of(epi_in, &epi))) return rc;
+  if ((rc = check_f32_path(path))) return rc;
+  if (!kernelStrides) return set_error(LASER_B200_EINVAL, "kernelStrides is NULL");
+  if (epi.bias && !epi.bias_per_row)
+    return set_error(LASER_B200_EINVAL, "a convolution's bias is one per output channel: bias_per_row must be 1");
+  if (g.B == 0) return LASER_B200_OK;
+  if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
+  const int64_t N = g.Cout, K = g.K(), P = g.outHW();
+  if (path == LASER_B200_PATH_AUTO) path = conv_auto_path(g, epi);
+  if (is_tc_mode(path) && P > 0x7fffffffLL / g.B)
+    return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: images * outH * outW must fit in int32");
+  epi.bias_per_row = 0;   // the output channels are the columns of C
+  const bool in_place = g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0;
+  ConvGeom gn = g;
+  gn.nhwc = true;
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  const int64_t per = batch_ws_per_problem(path, P, N, K, true, false, !in_place, false);
+  int64_t chunk = per > 0 ? c->batch_ws_bytes / per : g.B;
+  const int64_t max_m_blocks = 0x7fffffffLL / (16 * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N));
+  if (chunk > max_m_blocks * TC_BLOCK_M / P) chunk = max_m_blocks * TC_BLOCK_M / P;
+  if (chunk < 1) chunk = 1;
+  const int64_t image = g.H * g.W * g.C;
+  for (int64_t b0 = 0; b0 < g.B; b0 += chunk) {
+    const int64_t imgs = g.B - b0 < chunk ? g.B - b0 : chunk;
+    gn.B = imgs;
+    if ((rc = run_f32(*c, path, imgs * P, N, K, 1.0f, input + b0 * image, g.C, 1, kernel, kernelStrides[0], kernelStrides[1], 0.0f,
+                      output + b0 * P * N, N, 1, s, epi, nullptr, nullptr, 0, nullptr, false, nullptr, nullptr,
+                      in_place ? nullptr : &gn)))
+      return rc;
+  }
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
 
 template <typename T>
@@ -1978,6 +2042,7 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 
 #define LB200_BATCHED_FUSED_F32 batched_fused_entry
 #define LB200_CONV2D_FUSED_F32 conv2d_fused_dev
+#define LB200_CONV2D_NHWC_FUSED_F32 conv2d_nhwc_fused_dev
 #define LB200_CONV2D_FILTER_GRAD_F32 conv2d_filter_grad_dev
 #define LB200_CONV2D_INPUT_GRAD_F32 conv2d_input_grad_dev
 #include "capi_layers.inc"

@@ -89,6 +89,9 @@ struct ConvGeom {
   // dilation of the source (an im2col source only): the transposed geometry of the input gradient reads the output gradient
   // zero-dilated by the forward strides (split.cuh: Im2colGradSrc)
   int64_t dH = 1, dW = 1;
+  // channels-last images [B][H][W][C] (an im2col source only): the windows are rows in the (kh, kw, c) order of the NHWC
+  // forward call (split.cuh: Im2colNhwcSrc)
+  bool nhwc = false;
   __host__ __device__ int64_t K() const { return C * kH * kW; }
   __host__ __device__ int64_t outHW() const { return outH * outW; }
 };

@@ -573,8 +573,49 @@ struct Im2colGradSrc : Im2colSrc {
   int dH, dW;     // source dilation: the forward strides (1: none)
   OperandOp op;   // HAS_OP: the op on the source values
 };
-template <bool GRAD>
-using Im2colSrcOf = typename std::conditional<GRAD, Im2colGradSrc, Im2colSrc>::type;
+// ---- channels-last source: A of the NHWC forward convolution, prepared straight from the NHWC images ----------------
+// Row n * outHW + p -- image n of the launch, output pixel p = oh * outW + ow -- is the pixel's window in the filter matrix's
+// row order k = (kh * kW + kw) * C + ci: kH * kW runs of C contiguous floats,
+//   row[k] = in[((n * H + h) * W + w) * C + ci],  h = oh * sH - pH + kh,  w = ow * sW - pW + kw   (0 outside the image)
+// -- the im2col matrix of every image of the launch, one row per output pixel, K-major: the A operand of ONE product with the
+// [K][c_out] filter matrix, whose C is the NHWC output.  vec (C % 4 == 0 and a 16-byte aligned input): every float4 of a row
+// lies inside one tap, so it is one 16-byte load (or zeros) with the tap decoded once; otherwise element by element with
+// running (ci, kw, kh) counters.  A parameter struct of its own, so that Im2colSrc keeps its layout.
+struct Im2colNhwcSrc : Im2colSrc {
+  int vec;
+};
+inline Im2colNhwcSrc im2col_nhwc_src(const ConvGeom &g, const float *in) {
+  Im2colNhwcSrc q{};
+  static_cast<Im2colSrc &>(q) = im2col_src(g);
+  q.vec = g.C % 4 == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0;
+  return q;
+}
+// elements k .. k+3 of the channels-last window of output pixel (oh, ow) of image `img` (0 past K)
+__device__ __forceinline__ float4 nhwc_window_vec(const float *__restrict__ img, const Im2colNhwcSrc &q, int oh, int ow, int k) {
+  const int tap = k / q.C;
+  int ci = k - tap * q.C;
+  int kr = tap / q.kW, kc = tap - kr * q.kW;
+  if (q.vec) {   // k % 4 == 0 and C % 4 == 0: k .. k+3 are channels ci .. ci+3 of one tap
+    const int h = oh * q.sH - q.pH + kr, w = ow * q.sW - q.pW + kc;
+    if (k < q.K && static_cast<unsigned>(h) < static_cast<unsigned>(q.H) && static_cast<unsigned>(w) < static_cast<unsigned>(q.W))
+      return *reinterpret_cast<const float4 *>(img + (static_cast<int64_t>(h) * q.W + w) * q.C + ci);
+    return make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  }
+  float v[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const int h = oh * q.sH - q.pH + kr, w = ow * q.sW - q.pW + kc;
+    const bool inside = k + e < q.K && static_cast<unsigned>(h) < static_cast<unsigned>(q.H) &&
+                        static_cast<unsigned>(w) < static_cast<unsigned>(q.W);
+    v[e] = inside ? img[(static_cast<int64_t>(h) * q.W + w) * q.C + ci] : 0.0f;
+    if (++ci == q.C) { ci = 0; if (++kc == q.kW) { kc = 0; ++kr; } }
+  }
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+
+template <bool GRAD, bool NHWC = false>
+using Im2colSrcOf =
+    typename std::conditional<NHWC, Im2colNhwcSrc, typename std::conditional<GRAD, Im2colGradSrc, Im2colSrc>::type>::type;
 // elements k .. k+3 of the transposed window of pixel (oh, ow) of image `img` (aux: its aux image, HAS_OP)
 template <bool DIL, bool HAS_OP>
 __device__ __forceinline__ float4 grad_window_vec(const float *__restrict__ img, const float *__restrict__ aux, const Im2colGradSrc &q,
@@ -608,22 +649,24 @@ __device__ __forceinline__ float4 grad_window_vec(const float *__restrict__ img,
   }
   return make_float4(v[0], v[1], v[2], v[3]);
 }
-template <bool DIL, bool HAS_OP, typename Src>
+template <bool DIL, bool HAS_OP, bool NHWC, typename Src>
 __device__ __forceinline__ float4 source_vec(const float *__restrict__ img, const float *__restrict__ aux, const Src &q, int oh, int ow,
                                              int k) {
-  if constexpr (DIL || HAS_OP) return grad_window_vec<DIL, HAS_OP>(img, aux, q, oh, ow, k);
+  if constexpr (NHWC) return nhwc_window_vec(img, q, oh, ow, k);
+  else if constexpr (DIL || HAS_OP) return grad_window_vec<DIL, HAS_OP>(img, aux, q, oh, ow, k);
   else return window_vec(img, q, oh, ow, k);
 }
 
 // (F16X2: the row in registers next to the geometry needs more than the 64 registers of 4 CTAs per SM -- it spills there)
-// DIL / HAS_OP (an Im2colGradSrc): the transposed source of the input gradient, dilated / with an op; the forward call's
-// instantiations are <MODE, GROUP, false, false>.
-template <int MODE, int GROUP, bool DIL = false, bool HAS_OP = false>
+// DIL / HAS_OP (an Im2colGradSrc): the transposed source of the input gradient, dilated / with an op; NHWC (an Im2colNhwcSrc):
+// the channels-last source of the NHWC forward call; the NCHW forward call's instantiations are <MODE, GROUP, false, false>.
+template <int MODE, int GROUP, bool DIL = false, bool HAS_OP = false, bool NHWC = false>
 __global__ void __launch_bounds__(256, MODE == IM2COL_F16X2 ? 3 : 4)
-im2col_rows_kernel(const float *__restrict__ in, Im2colSrcOf<DIL || HAS_OP> q, int64_t images, float *__restrict__ dst,
+im2col_rows_kernel(const float *__restrict__ in, Im2colSrcOf<DIL || HAS_OP, NHWC> q, int64_t images, float *__restrict__ dst,
                    float *__restrict__ dst_lo, uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld,
                    uint32_t *__restrict__ absmax) {
   static_assert(GROUP == 32 || GROUP == 256, "a warp or the CTA per row");
+  static_assert(!NHWC || !(DIL || HAS_OP), "the channels-last source has no dilation or op");
   __shared__ uint32_t red[2][8];
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   const int tid = static_cast<int>(threadIdx.x) % GROUP;
@@ -642,7 +685,7 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrcOf<DIL || HAS_OP> q, i
     if constexpr (HAS_OP) aux = q.op.aux ? q.op.aux + n * q.image : nullptr;
     if constexpr (MODE != IM2COL_F16X2) {
       for (int idx = tid; idx < nvec; idx += GROUP) {
-        const float4 v = source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2);
+        const float4 v = source_vec<DIL, HAS_OP, NHWC>(img, aux, q, oh, ow, idx << 2);
         if constexpr (MODE == IM2COL_F32) {
           *reinterpret_cast<float4 *>(dst + r * ld + (idx << 2)) = v;
         } else {
@@ -662,12 +705,12 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrcOf<DIL || HAS_OP> q, i
       for (int i = 0; i < F16ROWS_MAXV; ++i) {
         const int idx = tid + i * GROUP;
         if (idx < nvec) {
-          v[i] = source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2);
+          v[i] = source_vec<DIL, HAS_OP, NHWC>(img, aux, q, oh, ow, idx << 2);
           m = max(max(m, finite_abs_bits(v[i].x)), max(finite_abs_bits(v[i].y), max(finite_abs_bits(v[i].z), finite_abs_bits(v[i].w))));
         }
       }
       for (int idx = tid + F16ROWS_MAXV * GROUP; idx < nvec; idx += GROUP) {
-        const float4 t = source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2);
+        const float4 t = source_vec<DIL, HAS_OP, NHWC>(img, aux, q, oh, ow, idx << 2);
         m = max(max(m, finite_abs_bits(t.x)), max(finite_abs_bits(t.y), max(finite_abs_bits(t.z), finite_abs_bits(t.w))));
       }
       float mf = __uint_as_float(m);     // non-negative finite: fmaxf orders them like the integers
@@ -690,7 +733,7 @@ im2col_rows_kernel(const float *__restrict__ in, Im2colSrcOf<DIL || HAS_OP> q, i
         if (idx < nvec) store_f16x2_vec(v[i], s, hrow, lrow, static_cast<int64_t>(idx) << 2);
       }
       for (int idx = tid + F16ROWS_MAXV * GROUP; idx < nvec; idx += GROUP)
-        store_f16x2_vec(source_vec<DIL, HAS_OP>(img, aux, q, oh, ow, idx << 2), s, hrow, lrow, static_cast<int64_t>(idx) << 2);
+        store_f16x2_vec(source_vec<DIL, HAS_OP, NHWC>(img, aux, q, oh, ow, idx << 2), s, hrow, lrow, static_cast<int64_t>(idx) << 2);
     }
   }
 }

@@ -151,6 +151,30 @@ def conv2d_fused(output, input, ishape, kernel, kshape, padding, strides, bias=N
                                                 ctypes.byref(epi), int(path), stream))
 
 
+def conv2d_nhwc_fused(output, input, ishape, kernel, kshape, padding, strides, bias=None, activation="none", path=PATH_AUTO,
+                      stream=None, kernel_strides=None):
+    """output_n <- act(conv(input_n, kernel) + bias) for every image n, on float32 DEVICE buffers in channels-last layout:
+    input dense NHWC [n, h, w, c], output dense NHWC [n, outH, outW, c_out]; ishape = (n, c, h, w) and kshape = (c_out, c_in,
+    kH, kW) as for conv2d_fused.  kernel: a 2-D device view [kH * kW * c_in, c_out] of the filter matrix, rows in (kh, kw, ci)
+    order -- e.g. a [kH, kW, c_in, c_out] tensor viewed as 2-D, or torch's channels_last weight viewed as [c_out, K] and
+    transposed; its element strides are read from the view (kernel_strides: for a pointer without strides).  bias: one per
+    output channel.  activation: none | relu | tanh | sigmoid.  One GEMM for the images, its A operand (the windows) prepared
+    straight from the images: no workspace."""
+    po, pi, pk = _dev_f32(output), _dev_f32(input), _dev_f32(kernel)
+    if kernel_strides is None:
+        kernel_strides = tuple(kernel.stride())
+    if len(kernel_strides) != 2:
+        raise ValueError("kernel must be a 2-D view [kH * kW * c_in, c_out]")
+    epi = Epilogue()
+    if bias is not None:
+        epi.bias = _dev_f32(bias)
+    epi.bias_per_row = 1
+    epi.activation = {"none": 0, "relu": 1, "tanh": 2, "sigmoid": 3}[activation]
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_nhwc_f32_fused_dev(po, pi, _i4(ishape), pk, _i4(kshape), _i2(kernel_strides), _i2(padding),
+                                                     _i2(strides), ctypes.byref(epi), int(path), stream))
+
+
 def conv2d_filter_grad_fused(grad_kernel, input, ishape, grad_output, kshape, padding, strides, alpha=1.0, beta=0.0, op=None,
                              aux=None, path=PATH_AUTO, stream=None):
     """grad_kernel <- alpha * sum_n op(grad_output_n) * im2col(input_n)^T + beta * grad_kernel on float32 DEVICE buffers: the

@@ -288,6 +288,11 @@ proc laser_b200_conv2d_im2col_f32*(output, input: ptr float32, ishape: ptr array
 proc laser_b200_conv2d_f32_fused_dev*(output, input: ptr float32, ishape: ptr array[4, int64], kernel: ptr float32,
                                       kshape: ptr array[4, int64], padding, strides: ptr array[2, int64],
                                       epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
+# the same in channels-last layout (conv2d_mec.nim): NHWC input and output, the filter matrix [kH*kW*c_in][c_out] read with
+# kernelStrides ({c_out, 1} for kernel_to_hwcc's layout); one GEMM over the windows prepared from the images
+proc laser_b200_conv2d_nhwc_f32_fused_dev*(output, input: ptr float32, ishape: ptr array[4, int64], kernel: ptr float32,
+                                           kshape: ptr array[4, int64], kernelStrides, padding, strides: ptr array[2, int64],
+                                           epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
 # its filter gradient (README.md:244-245, :251): grad_kernel <- alpha * sum_n op(grad_output_n) * im2col(input_n)^T +
 # beta * grad_kernel, one batch-reduced product whose B is prepared from the images; nil op = none
 proc laser_b200_conv2d_filter_grad_f32_fused_dev*(grad_kernel, input: ptr float32, ishape: ptr array[4, int64],
