@@ -501,6 +501,34 @@ int laser_b200_conv2d_filter_grad_f32_fused_dev(float *grad_kernel, const float 
                                                 const int64_t padding[2], const int64_t strides[2],
                                                 float alpha, float beta, const laser_b200_operand_op *op,
                                                 int path, void *stream);
+/* Filter gradient of the channels-last fused convolution (conv2d_nhwc_f32_fused_dev's layouts; the reference has no backward
+ * convolution):
+ *   Wmat[k][co] <- alpha * sum_{n,p} rows[n * P + p][k] * op(grad_output)[n * P + p][co] + beta * Wmat[k][co]
+ * with rows the NHWC forward call's windows, k = (kh * kW + kw) * c_in + ci, P = outH * outW, and ishape / kshape in the
+ * reference's tuple order as for conv2d_nhwc_f32_fused_dev.  input is dense NHWC [n][h][w][c]; grad_output is dense NHWC
+ * [n][outH][outW][c_out].  grad_kernel is the filter matrix written through the element strides kernelStrides = (over its rows,
+ * over output channels), the forward call's convention: {c_out, 1} for kernel_to_hwcc's [kH][kW][C_in][C_out], {1, kH * kW *
+ * c_in} for torch's channels_last weight [c_out][kH][kW][c_in].  op (NULL: none) is applied to grad_output; a derivative op's
+ * aux is dense NHWC of grad_output's shape, seen like A = op(grad_output)^T [c_out][n * P]: auxRowStride = 1, auxColStride =
+ * c_out.  beta = 1 accumulates across micro-batches.
+ *   NHWC stores the images end to end along n * P + p, so the call is ONE product (no batch is reduced), M = c_out, N = K,
+ *   K' = n * outH * outW: A = op(grad_output)^T read in place, B = the tap rows prepared straight from the images (16-byte loads
+ *   along the channels when c % 4 == 0 and input is 16-byte aligned), no workspace argument.  It runs as one chunk whatever
+ *   LASER_B200_BATCH_WS_MB says.  1 x 1 kernels with unit strides and no padding read input in place as the [c_in][n * h * w]
+ *   matrix.  grad_kernel is bit for bit what laser_b200_gemm_strided_f32_fused_dev gives on the same path for (M, N, K') =
+ *   (c_out, K, n * P), A = grad_output with strides (1, c_out) and op, B = the materialised tap rows [K][n * P], C = grad_kernel
+ *   with strides (kernelStrides[1], kernelStrides[0]).  On the exact path that is also conv2d_filter_grad_f32_fused_dev's result
+ *   on NCHW copies of the same data, permuted, bit for bit.
+ *   PATH_AUTO takes the path conv2d_filter_grad_f32_fused_dev takes for the same geometry.
+ *   n = 0: LASER_B200_OK, nothing launched, grad_kernel untouched.  n * outH * outW must fit in int32 on the tensor-core
+ *   paths (LASER_B200_EUNSUPPORTED otherwise, before anything is read).
+ *   LASER_B200_EINVAL, before anything is launched: geometry errors, kshape[1] != c_in, kernelStrides NULL, an unknown path
+ *   or op, a derivative op without aux or with other aux strides, a NULL pointer. */
+int laser_b200_conv2d_nhwc_filter_grad_f32_fused_dev(float *grad_kernel, const float *input, const int64_t ishape[4],
+                                                     const float *grad_output, const int64_t kshape[4],
+                                                     const int64_t kernelStrides[2], const int64_t padding[2],
+                                                     const int64_t strides[2], float alpha, float beta,
+                                                     const laser_b200_operand_op *op, int path, void *stream);
 /* Input gradient of the fused convolution (the reference has no backward convolution):
  *   grad_input <- alpha * conv_transpose(op(grad_output), kernel) + beta * grad_input
  * with the forward call's shapes: grad_input dense NCHW of shape ishape, grad_output dense NCHW [n][c_out][outH][outW]

@@ -584,20 +584,24 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
 // A dilated source (ConvGeom::dH, dW) or an op: the transposed source of the input gradient, the rows kernel's DIL / HAS_OP
 // instantiations (op applied to the values read, its aux dense like the images; not with `concat`).
 // A channels-last source (ConvGeom::nhwc): the windows of NHWC images in (kh, kw, c) order, the rows kernel's NHWC
-// instantiations; one problem, mn = images * outH * outW rows.
+// instantiations; one problem, mn = images * outH * outW rows.  Oriented as tap rows (ConvGeom::taps): mn = the taps, k = the
+// pixels of every image end to end (split.cuh: im2col_nhwc_tap_rows_kernel), F16X2 after an abs-max pass over the same tiles.
 int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst_lo, uint16_t *hb, uint16_t *lb, int64_t ld,
                 uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
   const Im2colSrc q = im2col_src(*o.conv);
   const Batch bt = batch_of(o);
   // the images of the launch: a batch of problems of outHW rows each (the NCHW sources), or one problem whose mn rows are the
-  // pixels of every image (the channels-last source, A of the NHWC forward call)
-  const int64_t images = o.concat ? bt.n : bt.n * (o.mn / q.outHW), rows = bt.n * o.mn;
-  const int64_t tiles = o.mn * ((ld + TAP_SEG - 1) / TAP_SEG);
+  // pixels of every image (the channels-last source, A of the NHWC forward call), or whose k columns are (the tap rows)
+  const int64_t images = o.conv->taps ? o.k / q.outHW : o.concat ? bt.n : bt.n * (o.mn / q.outHW), rows = bt.n * o.mn;
+  // the work items of a tap-row launch: tiles of TAP_SEG columns of one row (NCHW), of NHWC_TAPS rows x NHWC_PIX columns (NHWC)
+  const int64_t tiles = o.conv->taps ? ((o.mn + NHWC_TAPS - 1) / NHWC_TAPS) * ((ld + NHWC_PIX - 1) / NHWC_PIX)
+                                     : o.mn * ((ld + TAP_SEG - 1) / TAP_SEG);
   const float *in = static_cast<const float *>(o.ptr);
   const bool dil = o.conv->dH != 1 || o.conv->dW != 1;
   if (o.concat && (dil || op)) return set_error(LASER_B200_ECUDA, "internal: a concatenated im2col source has no dilation or op");
   if (o.conv->nhwc && (o.concat || dil || op))
     return set_error(LASER_B200_ECUDA, "internal: a channels-last im2col source is not concatenated, dilated or op'd");
+  if (o.conv->taps && !o.conv->nhwc) return set_error(LASER_B200_ECUDA, "internal: only a channels-last source has tap rows");
   auto launch = [&](auto m, auto absmax) {
     constexpr int MODE = decltype(m)::value, PER_SM = MODE == IM2COL_F16X2 ? 3 : 4;   // the kernel's launch bounds
     auto rows_kernel = [&](auto d, auto has_op, const auto &src) {
@@ -610,7 +614,10 @@ int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst
         im2col_rows_kernel<MODE, 256, DIL, HAS_OP, NHWC><<<grid_for(c, rows, PER_SM), 256, 0, s>>>(in, src, images, dst, dst_lo, hb,
                                                                                                 lb, ld, words);
     };
-    if (o.conv->nhwc) {
+    if (o.conv->taps) {
+      im2col_nhwc_tap_rows_kernel<MODE, decltype(absmax)::value><<<grid_for(c, tiles, NHWC_PER_SM), 256, 0, s>>>(
+          in, im2col_nhwc_src(*o.conv, in), images, dst, dst_lo, hb, lb, ld, words);
+    } else if (o.conv->nhwc) {
       rows_kernel(std::false_type(), std::false_type(), im2col_nhwc_src(*o.conv, in));
     } else if (o.concat) {
       im2col_tap_rows_kernel<MODE, decltype(absmax)::value><<<grid_for(c, tiles, 8), 256, 0, s>>>(in, q, images, dst, dst_lo, hb, lb,
@@ -631,7 +638,7 @@ int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst
     CHECK_LAUNCH();
     return LASER_B200_OK;
   };
-  if (mode == SPLIT_F16X2 && o.concat) {   // one word per tap row over every image
+  if (mode == SPLIT_F16X2 && (o.concat || o.conv->taps)) {   // one word per tap row over every image
     CUDA_TRY(cudaMemsetAsync(words, 0, static_cast<size_t>(o.mn) * sizeof(uint32_t), s));
     const int rc = launch(std::integral_constant<int, IM2COL_F16X2>(), std::true_type());
     if (rc) return rc;
@@ -1096,7 +1103,8 @@ int simt_run(Ctx &c, const Operand &oa, const Operand &ob, float alpha, float be
 //     batch shares, op included, is one problem, prepared once.  The problems' C bs->C apart.
 //   concat: the sum of the batch's products into one C, one product over the operands concatenated along k
 //     (Operand::concat; bs->C unused).
-//   convB: B is an im2col source, the images at B bs->B floats apart (rsB, csB unused).
+//   convB: B is an im2col source, the images at B bs->B floats apart (rsB, csB unused).  A channels-last one as tap rows
+//     (ConvGeom::taps): N = the taps, K = images * outH * outW pixels of the images at B (a single problem).
 //   convA: A is a channels-last im2col source (ConvGeom::nhwc), M = images * outH * outW rows of the images at A (rsA, csA
 //     unused; a single problem).
 int run_f32(Ctx &c, int path, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA, const float *B,
@@ -1507,6 +1515,47 @@ int conv2d_filter_grad_dev(float *grad_kernel, const float *input, const ConvGeo
   const laser_b200_batch_strides bs{M * P, image, 0, M * P, 0};
   return batch_reduce_dev(g.B, M, N, P, alpha, grad_output, P, 1, input, 1, P, beta, grad_kernel, N, 1, &bs, opA, nullptr, Epilogue(),
                           path, stream, in_place ? nullptr : &g);
+}
+
+// laser_b200_conv2d_nhwc_filter_grad_f32_fused_dev (capi_layers.inc checks the geometry): NHWC images and gradients, ONE product
+//   dWmat[k][co] <- alpha * sum_j rows[j][k] * op(dY)[j][co] + beta * dWmat[k][co],  j = n * P + p over every image
+// with M = Cout, N = K = kH * kW * C, K' = n * P: A = op(dY)^T, the [Cout][n * P] view of the NHWC gradients (strides (1, Cout),
+// MN-major; the op's aux laid out the same way), B = the images as channels-last tap rows (ConvGeom::taps), C = the filter matrix
+// through kernelStrides (C[co][k] at co * kernelStrides[1] + k * kernelStrides[0]).  NHWC stores the images end to end along j,
+// so no batch is reduced.  1 x 1 kernels with unit strides and no padding: B is the images read in place as [C][n * H * W].
+// One chunk always: chunks would round dW between them.
+int conv2d_nhwc_filter_grad_dev(float *grad_kernel, const float *input, const ConvGeom &g, const float *grad_output,
+                                const int64_t kernelStrides[2], float alpha, float beta, const laser_b200_operand_op *op_in, int path,
+                                void *stream) {
+  int rc;
+  if ((rc = check_f32_path(path))) return rc;
+  if (!kernelStrides) return set_error(LASER_B200_EINVAL, "kernelStrides is NULL");
+  OperandOp op;
+  const OperandOp *opA;
+  if ((rc = operand_op_of(op_in, false, &op, &opA))) return rc;
+  const int64_t M = g.Cout, N = g.K(), P = g.outHW();
+  if (opA && opA->aux && (opA->aux_sr != 1 || opA->aux_sc != M))
+    return set_error(LASER_B200_EINVAL, "the aux tensor of op %d must be dense NHWC like grad_output: strides (1, %lld), not (%lld, %lld)",
+                     opA->op, (long long)M, (long long)opA->aux_sr, (long long)opA->aux_sc);
+  if (g.B == 0) return LASER_B200_OK;
+  if (!grad_kernel || !input || !grad_output) return set_error(LASER_B200_EINVAL, "null pointer");
+  if (P > INT64_MAX / g.B) return set_error(LASER_B200_EUNSUPPORTED, "images * outH * outW overflows int64");
+  const int64_t Kr = g.B * P;
+  // PATH_AUTO: as the NCHW filter gradient decides for the same geometry (batch_reduce_dev over K' = n * P)
+  if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, Kr, Epilogue(), /*operand_op=*/true);
+  if (is_tc_mode(path) && Kr > 0x7fffffffLL)
+    return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: images * outH * outW must fit in int32");
+  const bool in_place = g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0;
+  ConvGeom gt = g;
+  gt.nhwc = gt.taps = true;
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  if ((rc = run_f32(*c, path, M, N, Kr, alpha, grad_output, 1, M, input, g.C, 1, beta, grad_kernel, kernelStrides[1], kernelStrides[0],
+                    s, Epilogue(), opA, nullptr, 0, nullptr, false, in_place ? nullptr : &gt)))
+    return rc;
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -2044,6 +2093,7 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 #define LB200_CONV2D_FUSED_F32 conv2d_fused_dev
 #define LB200_CONV2D_NHWC_FUSED_F32 conv2d_nhwc_fused_dev
 #define LB200_CONV2D_FILTER_GRAD_F32 conv2d_filter_grad_dev
+#define LB200_CONV2D_NHWC_FILTER_GRAD_F32 conv2d_nhwc_filter_grad_dev
 #define LB200_CONV2D_INPUT_GRAD_F32 conv2d_input_grad_dev
 #include "capi_layers.inc"
 #include "capi_multi.inc"

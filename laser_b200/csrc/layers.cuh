@@ -92,6 +92,9 @@ struct ConvGeom {
   // channels-last images [B][H][W][C] (an im2col source only): the windows are rows in the (kh, kw, c) order of the NHWC
   // forward call (split.cuh: Im2colNhwcSrc)
   bool nhwc = false;
+  // with nhwc: the windows oriented as tap rows (an im2col source only) -- the operand's mn is the tap (kh, kw, c), its k the
+  // pixel index n * outH * outW + p: B of the NHWC filter gradient (split.cuh: im2col_nhwc_tap_rows_kernel)
+  bool taps = false;
   __host__ __device__ int64_t K() const { return C * kH * kW; }
   __host__ __device__ int64_t outHW() const { return outH * outW; }
 };

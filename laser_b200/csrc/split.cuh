@@ -819,6 +819,136 @@ im2col_tap_rows_kernel(const float *__restrict__ in, Im2colSrc q, int64_t images
   }
 }
 
+// ---- channels-last tap rows: the filter-gradient B of an NHWC convolution, prepared straight from the NHWC images -------
+// Tap row k = (kh * kW + kw) * C + ci -- the filter matrix's row order -- holds the tap's value at every output pixel of every
+// image of the launch, end to end along the NHWC gradients' row index j = n * P + p (P = outHW, p = oh * outW + ow):
+//   row[k][j] = in[((n * H + h) * W + w) * C + ci],  h = oh * sH - pH + kh,  w = ow * sW - pW + kw   (0 outside the image)
+// -- the NHWC forward's window rows transposed: the K-major B of ONE product dWmat^T = op(dY)^T * rows.  Consecutive columns of
+// a row lie sW * C floats apart in the images, so a work item is a tile of NHWC_TAPS consecutive taps x NHWC_PIX consecutive
+// columns, transposed through shared memory: the reads go along the channels (vec: one 16-byte load per 4 taps of one pixel,
+// a warp reading 4 pixels x 32 taps; otherwise element by element), the writes along the pixels, a warp per tap row segment.
+// The pixels (n, oh, ow) are decoded once per column and the taps (kh, kw, ci) once per tap, per tile.  The modes write what
+// im2col_tap_rows_kernel's write over the same rows, bit for bit (F16X2: the words come from an ABSMAX launch of the same tiles
+// first, zeroed by the host, one atomicMax per tap per tile).  Every column up to ld is written (zeros past n * P).
+// Shared tile [tap][column]: the float4 slot of columns 4s .. 4s+3 of tap t sits at slot s ^ (t / 4), so that the staging
+// stores (4 columns x 8 tap quads per warp) and the row reads (one float4 per lane) are both free of bank conflicts.
+// NHWC_PER_SM CTAs per SM: the launch bounds the registers to what that many CTAs leave, and the host sizes the grid to it;
+// six is also what the 37 KB of shared memory of a 256-column tile allows.  NHWC_PIX = 256 was the fastest of 64, 128 and 256
+// on an H100 (DESIGN.md section 4); a wider tile no longer fits the 48 KB of static shared memory.
+constexpr int NHWC_TAPS = 32;     // taps of one tile
+constexpr int NHWC_PIX = 256;     // columns of one tile
+constexpr int NHWC_PER_SM = 6;    // resident CTAs per SM
+template <int MODE, bool ABSMAX = false>
+__global__ void __launch_bounds__(256, NHWC_PER_SM)
+im2col_nhwc_tap_rows_kernel(const float *__restrict__ in, Im2colNhwcSrc q, int64_t images, float *__restrict__ dst,
+                            float *__restrict__ dst_lo, uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld,
+                            uint32_t *__restrict__ absmax) {
+  static_assert(!ABSMAX || MODE == IM2COL_F16X2, "only the f16x2 rows carry a scale word");
+  static_assert(NHWC_TAPS == 32 && NHWC_PIX % 32 == 0 && NHWC_PIX >= 32 && NHWC_PIX + NHWC_TAPS <= 512,
+                "8 tap quads per column, 8 warps x 4 rows, whole float4 slots for the swizzle, two decode items per thread at most");
+  __shared__ __align__(16) float tile[NHWC_TAPS * NHWC_PIX];
+  __shared__ int64_t col_off[NHWC_PIX];        // the pixel's window corner (n, h0, w0) in floats from `in`
+  __shared__ int col_h[NHWC_PIX], col_w[NHWC_PIX];
+  __shared__ int tap_off[NHWC_TAPS], tap_h[NHWC_TAPS], tap_w[NHWC_TAPS];
+  ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
+  const int tid = static_cast<int>(threadIdx.x), lane = tid & 31, warp = tid >> 5;
+  const int64_t cols = images * q.outHW;
+  const int64_t tap_tiles = (q.K + NHWC_TAPS - 1) / NHWC_TAPS, col_tiles = (ld + NHWC_PIX - 1) / NHWC_PIX;
+  // the tap tiles of one column block are neighbours in the loop: CTAs running together read the same pixels' windows
+  for (int64_t it = blockIdx.x; it < tap_tiles * col_tiles; it += gridDim.x) {
+    const int64_t cb = it / tap_tiles;
+    const int t0 = static_cast<int>(it - cb * tap_tiles) * NHWC_TAPS;
+    const int64_t j0 = cb * NHWC_PIX;
+    for (int d = tid; d < NHWC_PIX + NHWC_TAPS; d += 256) {
+      if (d < NHWC_PIX) {
+        const int64_t j = j0 + d;
+        int h0 = -(1 << 30), w0 = 0;   // past the images: no tap is inside
+        int64_t off = 0;
+        if (j < cols) {
+          const int64_t n = j / q.outHW;
+          const int p = static_cast<int>(j - n * q.outHW), oh = p / q.outW, ow = p - oh * q.outW;
+          h0 = oh * q.sH - q.pH;
+          w0 = ow * q.sW - q.pW;
+          off = n * q.image + (static_cast<int64_t>(h0) * q.W + w0) * q.C;
+        }
+        col_h[d] = h0; col_w[d] = w0; col_off[d] = off;
+      } else {
+        const int t = t0 + d - NHWC_PIX;
+        int kr = 0, kc = 0, off = 0;   // (past K: every read is skipped)
+        if (t < q.K) {
+          const int tap = t / q.C, ci = t - tap * q.C;
+          kr = tap / q.kW;
+          kc = tap - kr * q.kW;
+          off = (kr * q.W + kc) * q.C + ci;
+        }
+        tap_h[d - NHWC_PIX] = kr; tap_w[d - NHWC_PIX] = kc; tap_off[d - NHWC_PIX] = off;
+      }
+    }
+    __syncthreads();   // (also: every warp has read the previous tile out of `tile`)
+#pragma unroll
+    for (int i = 0; i < NHWC_TAPS * NHWC_PIX / 4 / 256; ++i) {
+      const int item = tid + 256 * i, cl = item >> 3, tq = item & 7;   // column cl, taps 4 tq .. 4 tq + 3 of the tile
+      const int h0 = col_h[cl], w0 = col_w[cl];
+      const float *px = in + col_off[cl];
+      float v[4];
+      if (q.vec) {   // C % 4 == 0: the four taps are channels ci .. ci + 3 of one (kh, kw), K % 4 == 0
+        const int t = 4 * tq;
+        const int h = h0 + tap_h[t], w = w0 + tap_w[t];
+        float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (t0 + t < q.K && static_cast<unsigned>(h) < static_cast<unsigned>(q.H) && static_cast<unsigned>(w) < static_cast<unsigned>(q.W))
+          x = *reinterpret_cast<const float4 *>(px + tap_off[t]);
+        v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
+      } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int t = 4 * tq + e;
+          const int h = h0 + tap_h[t], w = w0 + tap_w[t];
+          const bool inside = t0 + t < q.K && static_cast<unsigned>(h) < static_cast<unsigned>(q.H) &&
+                              static_cast<unsigned>(w) < static_cast<unsigned>(q.W);
+          v[e] = inside ? px[tap_off[t]] : 0.0f;
+        }
+      }
+      const int slot = (((cl >> 2) ^ tq) << 2) + (cl & 3);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) tile[(4 * tq + e) * NHWC_PIX + slot] = v[e];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < NHWC_TAPS / 8; ++i) {
+      const int r = warp + 8 * i, t = t0 + r;
+      if (t >= q.K) break;   // (uniform over the warp)
+      uint32_t m = 0u;
+      for (int c4 = lane; c4 < NHWC_PIX / 4; c4 += 32) {   // this lane's float4 of the row segment
+        const int64_t j = j0 + 4 * c4;
+        const float4 x = *reinterpret_cast<const float4 *>(tile + r * NHWC_PIX + ((c4 ^ (r >> 2)) << 2));
+        if constexpr (ABSMAX) {   // (columns past ld are zeros)
+          m = max(max(m, max(finite_abs_bits(x.x), finite_abs_bits(x.y))), max(finite_abs_bits(x.z), finite_abs_bits(x.w)));
+        } else if (j < ld) {
+          if constexpr (MODE == IM2COL_F32) {
+            *reinterpret_cast<float4 *>(dst + t * ld + j) = x;
+          } else if constexpr (MODE == IM2COL_TF32) {
+            float4 h, l;
+            h.x = tf32_rna(x.x); l.x = tf32_lo(x.x, h.x);
+            h.y = tf32_rna(x.y); l.y = tf32_lo(x.y, h.y);
+            h.z = tf32_rna(x.z); l.z = tf32_lo(x.z, h.z);
+            h.w = tf32_rna(x.w); l.w = tf32_lo(x.w, h.w);
+            *reinterpret_cast<float4 *>(dst + t * ld + j) = h;
+            *reinterpret_cast<float4 *>(dst_lo + t * ld + j) = l;
+          } else {
+            store_f16x2_vec(x, f16x2_scale(absmax[t]), hb + t * ld, lb + t * ld, j);
+          }
+        }
+      }
+      if constexpr (ABSMAX) {   // every lane takes part, with 0 where it had no column
+        float mf = __uint_as_float(m);   // non-negative finite: fmaxf orders them like the integers
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mf = fmaxf(mf, __shfl_xor_sync(0xffffffffu, mf, o));
+        if (lane == 0) atomicMax(absmax + t, __float_as_uint(mf));
+      }
+    }
+  }
+}
+
 // dst[r*ld + c] = src[r*sr + c*sc] for r < R, c < Cc.  32 x 32 tiles through shared
 // memory so that both the gather (along whichever source stride is smaller) and the
 // store (along c) are coalesced.  SPLIT: also write lo (fp32 only).

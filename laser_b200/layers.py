@@ -11,6 +11,8 @@
                                                   GEMM's operand preparation (README.md:251)
     conv2d_filter_grad_fused                      its filter gradient, derivative op on grad_output and the window gather
                                                   folded into the operand preparation (README.md:244-245, :251)
+    conv2d_nhwc_filter_grad_fused                 the filter gradient of conv2d_nhwc_fused: NHWC images and gradients, the
+                                                  tap rows transposed out of the images in the operand preparation
     conv2d_input_grad_fused                       its input gradient, the transposed window gather over grad_output folded
                                                   into the operand preparation
     gemm_strided_batched                          (roadmap item of the reference, README.md:253-263)
@@ -195,6 +197,33 @@ def conv2d_filter_grad_fused(grad_kernel, input, ishape, grad_output, kshape, pa
     check(lib().laser_b200_conv2d_filter_grad_f32_fused_dev(pw, pi, _i4(ishape), pg, _i4(kshape), _i2(padding), _i2(strides),
                                                             float(alpha), float(beta), ctypes.byref(o) if o is not None else None,
                                                             int(path), stream))
+
+
+def conv2d_nhwc_filter_grad_fused(grad_kernel, input, ishape, grad_output, kshape, padding, strides, alpha=1.0, beta=0.0, op=None,
+                                  aux=None, path=PATH_AUTO, stream=None, kernel_strides=None):
+    """grad_kernel <- alpha * sum_{n,p} rows[n * P + p]^T * op(grad_output)[n * P + p] + beta * grad_kernel on float32 DEVICE
+    buffers: the filter gradient of conv2d_nhwc_fused (input dense NHWC [n, h, w, c], grad_output dense NHWC [n, outH, outW,
+    c_out]).  grad_kernel: a 2-D device view [kH * kW * c_in, c_out] of the filter matrix, rows in (kh, kw, ci) order, whose
+    element strides are read as conv2d_nhwc_fused reads them (kernel_strides: for a pointer without strides).  op: None or
+    relu | tanh | sigmoid | relu_grad | tanh_grad | sigmoid_grad, applied to grad_output; a derivative takes `aux`, a dense NHWC
+    tensor of grad_output's shape (the forward output).  beta=1 accumulates across micro-batches.  One product whose B operand
+    (the tap rows) is prepared straight from the images: no conversion to NCHW, no workspace."""
+    pw, pi, pg = _dev_f32(grad_kernel), _dev_f32(input), _dev_f32(grad_output)
+    if kernel_strides is None:
+        kernel_strides = tuple(grad_kernel.stride())
+    if len(kernel_strides) != 2:
+        raise ValueError("grad_kernel must be a 2-D view [kH * kW * c_in, c_out]")
+    o = None
+    if op is not None:
+        o = OperandOp()
+        o.op = OP_NAMES[op]
+        if aux is not None:
+            o.aux = _dev_f32(aux)
+            o.auxRowStride, o.auxColStride = 1, kshape[0]
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_nhwc_filter_grad_f32_fused_dev(pw, pi, _i4(ishape), pg, _i4(kshape), _i2(kernel_strides),
+                                                                 _i2(padding), _i2(strides), float(alpha), float(beta),
+                                                                 ctypes.byref(o) if o is not None else None, int(path), stream))
 
 
 def conv2d_input_grad_fused(grad_input, ishape, grad_output, kernel, kshape, padding, strides, alpha=1.0, beta=0.0, op=None,

@@ -299,6 +299,12 @@ proc laser_b200_conv2d_filter_grad_f32_fused_dev*(grad_kernel, input: ptr float3
                                                   grad_output: ptr float32, kshape: ptr array[4, int64],
                                                   padding, strides: ptr array[2, int64], alpha, beta: float32,
                                                   op: ptr LaserB200OperandOp, path: cint, stream: pointer): cint
+# the filter gradient of the channels-last call: grad_kernel (the filter matrix [kH*kW*c_in][c_out] through kernelStrides) <-
+# alpha * rows^T * op(grad_output) + beta * grad_kernel over every NHWC image at once, B's tap rows prepared from the images
+proc laser_b200_conv2d_nhwc_filter_grad_f32_fused_dev*(grad_kernel, input: ptr float32, ishape: ptr array[4, int64],
+                                                       grad_output: ptr float32, kshape: ptr array[4, int64],
+                                                       kernelStrides, padding, strides: ptr array[2, int64], alpha, beta: float32,
+                                                       op: ptr LaserB200OperandOp, path: cint, stream: pointer): cint
 # its input gradient: grad_input <- alpha * conv_transpose(op(grad_output), kernel) + beta * grad_input, the forward product
 # over the rotated filters and a B prepared from grad_output; nil op = none
 proc laser_b200_conv2d_input_grad_f32_fused_dev*(grad_input: ptr float32, ishape: ptr array[4, int64],
