@@ -553,6 +553,37 @@ int laser_b200_conv2d_input_grad_f32_fused_dev(float *grad_input, const int64_t 
                                                const float *kernel, const int64_t kshape[4], const int64_t padding[2],
                                                const int64_t strides[2], float alpha, float beta,
                                                const laser_b200_operand_op *op, int path, void *stream);
+/* Input gradient of the channels-last fused convolution (conv2d_nhwc_f32_fused_dev's layouts; the reference has no backward
+ * convolution):
+ *   grad_input[j][ci] <- alpha * sum_k' R[j][k'] * W'^T[ci][k'] + beta * grad_input[j][ci],  j = n * H * W + ih * W + iw
+ * with T = kH * kW, k' = (kh' * kW + kw') * c_out + co, W'^T[ci][k'] = Wmat[(T - 1 - (kh' * kW + kw')) * c_in + ci][co], and
+ * R[j][k'] = op(grad_output)[n][h / sH][w / sW][co] where h = ih - (kH - 1 - pH) + kh' >= 0, h % sH == 0 and h / sH < outH
+ * (columns likewise), else 0 (a hole is 0, never op(0)).  ishape / kshape are in the reference's tuple order as for
+ * conv2d_nhwc_f32_fused_dev.  grad_input is dense NHWC [n][h][w][c_in]; grad_output is dense NHWC [n][outH][outW][c_out].
+ * kernel is the filter matrix Wmat[(kh * kW + kw) * c_in + ci][co] read through kernelStrides, the forward call's convention:
+ * {c_out, 1} for kernel_to_hwcc's [kH][kW][C_in][C_out], {1, kH * kW * c_in} for torch's channels_last weight, or any other.
+ * op (NULL: none) is applied to grad_output with conv2d_nhwc_filter_grad_f32_fused_dev's op set; a derivative op's aux is
+ * dense NHWC of grad_output's shape, seen like grad_output as [n * outH * outW][c_out]: auxRowStride = c_out, auxColStride = 1.
+ * beta = 1 accumulates into an existing gradient.  No bias gradient.
+ *   The images of a chunk (LASER_B200_BATCH_WS_MB) are ONE product, M = n * H * W, N = c_in, K' = T * c_out: A = R prepared
+ *   straight from grad_output (16-byte loads along the channels when c_out % 4 == 0 and grad_output and the aux are 16-byte
+ *   aligned), B = W'^T (written once per call into library workspace), C = grad_input.  grad_input is bit for bit what
+ *   laser_b200_gemm_strided_f32_fused_dev gives on the same path for (M, N, K') = (n * H * W, c_in, K'), A = the materialised
+ *   rows R, B = W'^T, C = grad_input with strides (c_in, 1); chunks give the bits of one.  At stride 1 with pH <= kH - 1,
+ *   without op, alpha = 1 and beta = 0, that is conv2d_nhwc_f32_fused_dev over (grad_output, W'^T as a [c_in][K'] buffer
+ *   with kernelStrides (1, K'), padding kH - 1 - pH) on the same path.  The exact path sums K' in (tap, co) order, so it is
+ *   not bit for bit conv2d_input_grad_f32_fused_dev's result, which sums in (co, tap) order.  1 x 1 kernels with unit
+ *   strides and no padding are the plain product op(grad_output) * Wmat^T, grad_output read in place as [n * P][c_out] and
+ *   kernel through its strides: no copy.
+ *   PATH_AUTO takes the path conv2d_input_grad_f32_fused_dev takes for the same geometry.
+ *   n = 0: LASER_B200_OK, nothing launched, grad_input untouched.  c_out * kH * kW must fit in int32, and on the tensor-core
+ *   paths n * H * W too (LASER_B200_EUNSUPPORTED otherwise, before anything is read).
+ *   LASER_B200_EINVAL, before anything is launched: geometry errors, kshape[1] != c_in, kernelStrides NULL, an unknown path
+ *   or op, a derivative op without aux or with other aux strides, a NULL pointer. */
+int laser_b200_conv2d_nhwc_input_grad_f32_fused_dev(float *grad_input, const int64_t ishape[4], const float *grad_output,
+                                                    const float *kernel, const int64_t kshape[4], const int64_t kernelStrides[2],
+                                                    const int64_t padding[2], const int64_t strides[2], float alpha, float beta,
+                                                    const laser_b200_operand_op *op, int path, void *stream);
 /* host pointers, synchronous, library-owned workspace */
 int laser_b200_conv2d_im2col_f32(float *output, const float *input, const int64_t ishape[4],
                                  const float *kernel, const int64_t kshape[4], const int64_t padding[2],

@@ -128,7 +128,8 @@ struct Ctx {
   Buffer splitk;     // split-K partial-sum planes
   Buffer bpanels;    // row-sharded products: B prepared, panel-major (capi_multi.inc: rowshard_prepared)
   Buffer layer_ws;   // im2col workspace of the host-pointer convolution
-  Buffer tfilt;      // the convolution input gradient's rotated filters W' (conv2d_input_grad_dev), under tfilt_mu for a whole call
+  Buffer tfilt;      // the input gradients' rotated filters, under tfilt_mu for a whole call: W' (conv2d_input_grad_dev) or W'^T
+                     // (conv2d_nhwc_input_grad_dev)
   Buffer f16s;       // F16X3 mode: fp32 bits of max_k |a| per row of A (words [0, M)) and of max_k |b| per column of B (from
                      // f16_b_off on), written and read on the device
   Buffer sched;      // kSchedSlots x {next unit, CTAs done}: the kernel re-zeroes its slot when it ends
@@ -136,7 +137,8 @@ struct Ctx {
   cudaEvent_t ws_free = nullptr;  // recorded after the last kernel that reads ws[]
   std::mutex mu;       // workspace + tensor-map construction
   std::mutex host_mu;  // staging buffers of the host-pointer entry points
-  std::mutex tfilt_mu; // tfilt: written once per input-gradient call, read by every chunk's product (each takes mu itself)
+  std::mutex tfilt_mu; // tfilt: written once per call of either input gradient, read by every chunk's product (each takes mu
+                       // itself)
   std::atomic<bool> ready{false};
 };
 
@@ -584,7 +586,9 @@ int f16x2_col_split(Ctx &c, const float *src, int64_t R, int64_t Cc, int64_t src
 // A dilated source (ConvGeom::dH, dW) or an op: the transposed source of the input gradient, the rows kernel's DIL / HAS_OP
 // instantiations (op applied to the values read, its aux dense like the images; not with `concat`).
 // A channels-last source (ConvGeom::nhwc): the windows of NHWC images in (kh, kw, c) order, the rows kernel's NHWC
-// instantiations; one problem, mn = images * outH * outW rows.  Oriented as tap rows (ConvGeom::taps): mn = the taps, k = the
+// instantiations; one problem, mn = images * outH * outW rows; dilated or op'd, the channels-last transposed source of the
+// NHWC input gradient (Im2colNhwcGradSrc; vector loads only when the aux is 16-byte aligned too).  Oriented as tap rows
+// (ConvGeom::taps, neither dilated nor op'd): mn = the taps, k = the
 // pixels of every image end to end (split.cuh: im2col_nhwc_tap_rows_kernel), F16X2 after an abs-max pass over the same tiles.
 int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst_lo, uint16_t *hb, uint16_t *lb, int64_t ld,
                 uint32_t *words, cudaStream_t s, const OperandOp *op = nullptr) {
@@ -599,14 +603,14 @@ int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst
   const float *in = static_cast<const float *>(o.ptr);
   const bool dil = o.conv->dH != 1 || o.conv->dW != 1;
   if (o.concat && (dil || op)) return set_error(LASER_B200_ECUDA, "internal: a concatenated im2col source has no dilation or op");
-  if (o.conv->nhwc && (o.concat || dil || op))
-    return set_error(LASER_B200_ECUDA, "internal: a channels-last im2col source is not concatenated, dilated or op'd");
-  if (o.conv->taps && !o.conv->nhwc) return set_error(LASER_B200_ECUDA, "internal: only a channels-last source has tap rows");
+  if (o.conv->nhwc && o.concat) return set_error(LASER_B200_ECUDA, "internal: a channels-last im2col source is not concatenated");
+  if (o.conv->taps && (!o.conv->nhwc || dil || op))
+    return set_error(LASER_B200_ECUDA, "internal: only a channels-last source without dilation or op has tap rows");
   auto launch = [&](auto m, auto absmax) {
     constexpr int MODE = decltype(m)::value, PER_SM = MODE == IM2COL_F16X2 ? 3 : 4;   // the kernel's launch bounds
     auto rows_kernel = [&](auto d, auto has_op, const auto &src) {
       constexpr bool DIL = decltype(d)::value, HAS_OP = decltype(has_op)::value;
-      constexpr bool NHWC = std::is_same<typename std::decay<decltype(src)>::type, Im2colNhwcSrc>::value;
+      constexpr bool NHWC = std::is_base_of<Im2colNhwcSrc, typename std::decay<decltype(src)>::type>::value;
       if (ld <= 4 * 32 * F16ROWS_MAXV)
         im2col_rows_kernel<MODE, 32, DIL, HAS_OP, NHWC><<<grid_for(c, (rows + 7) / 8, PER_SM), 256, 0, s>>>(in, src, images, dst,
                                                                                                          dst_lo, hb, lb, ld, words);
@@ -617,6 +621,16 @@ int im2col_rows(Ctx &c, const Operand &o, SplitMode mode, float *dst, float *dst
     if (o.conv->taps) {
       im2col_nhwc_tap_rows_kernel<MODE, decltype(absmax)::value><<<grid_for(c, tiles, NHWC_PER_SM), 256, 0, s>>>(
           in, im2col_nhwc_src(*o.conv, in), images, dst, dst_lo, hb, lb, ld, words);
+    } else if (o.conv->nhwc && (dil || op)) {
+      Im2colNhwcGradSrc gq{};
+      static_cast<Im2colNhwcSrc &>(gq) = im2col_nhwc_src(*o.conv, in);
+      gq.vec = gq.vec && (!op || !op->aux || (reinterpret_cast<uintptr_t>(op->aux) & 15) == 0);
+      gq.dH = static_cast<int>(o.conv->dH);
+      gq.dW = static_cast<int>(o.conv->dW);
+      if (op) gq.op = *op;
+      if (dil && op) rows_kernel(std::true_type(), std::true_type(), gq);
+      else if (dil) rows_kernel(std::true_type(), std::false_type(), gq);
+      else rows_kernel(std::false_type(), std::true_type(), gq);
     } else if (o.conv->nhwc) {
       rows_kernel(std::false_type(), std::false_type(), im2col_nhwc_src(*o.conv, in));
     } else if (o.concat) {
@@ -1389,12 +1403,39 @@ int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const
   return conv_windows_dev(g, 1.0f, kernel, g.K(), 1, input, 0.0f, output, nullptr, epi, path, stream);
 }
 
+// The product of both channels-last convolution entries, over the NHWC images `src` (a geometry with nhwc set) at A:
+//   C[n * P + p][j] <- epi(alpha * sum_k A(n * P + p, k) * B[k][j] + beta * C[n * P + p][j]),  P = src.outHW(), K = src.K()
+// A the images' windows (split.cuh: Im2colNhwcSrc, dilated or op'd Im2colNhwcGradSrc), or with in_place the images themselves
+// read as [n * P][K]; opA applied to the values read, its aux laid out like the images.  B [K][N] through (rsB, csB); C dense
+// [n * P][N].  Chunks of whole images under LASER_B200_BATCH_WS_MB, the tile count of each in int32, one preparation and one
+// GEMM launch sequence each; the images do not sum into each other, so chunks give the bits of one.
+int conv_nhwc_chunks(Ctx &c, int path, const ConvGeom &src, int64_t N, float alpha, const float *A, const float *B, int64_t rsB,
+                     int64_t csB, float beta, float *C, cudaStream_t s, const Epilogue &epi, const OperandOp *opA, bool in_place) {
+  const int64_t K = src.K(), P = src.outHW(), image = src.H * src.W * src.C;
+  const int64_t per = batch_ws_per_problem(path, P, N, K, true, false, !in_place || opA, false);
+  int64_t chunk = per > 0 ? c.batch_ws_bytes / per : src.B;
+  const int64_t max_m_blocks = 0x7fffffffLL / (16 * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N));
+  if (chunk > max_m_blocks * TC_BLOCK_M / P) chunk = max_m_blocks * TC_BLOCK_M / P;
+  if (chunk < 1) chunk = 1;
+  ConvGeom gc = src;
+  int rc;
+  for (int64_t b0 = 0; b0 < src.B; b0 += chunk) {
+    const int64_t imgs = src.B - b0 < chunk ? src.B - b0 : chunk;
+    gc.B = imgs;
+    OperandOp ca;
+    if (opA) { ca = *opA; if (ca.aux) ca.aux += b0 * image; }
+    if ((rc = run_f32(c, path, imgs * P, N, K, alpha, A + b0 * image, src.C, 1, B, rsB, csB, beta, C + b0 * P * N, N, 1, s, epi,
+                      opA ? &ca : nullptr, nullptr, 0, nullptr, false, nullptr, nullptr, in_place ? nullptr : &gc)))
+      return rc;
+  }
+  return LASER_B200_OK;
+}
+
 // laser_b200_conv2d_nhwc_f32_fused_dev (capi_layers.inc checks the geometry): NHWC images, one product for the images of a chunk,
 //   output[n * P + p][co] = act(sum_k rows[n * P + p][k] * Wmat[k][co] + bias[co]),  P = outH * outW
 // A = the images as a channels-last im2col source (one row per output pixel, K-major), B = the filter matrix [K][c_out] read
 // with its strides (kernelStrides[0] over k, [1] over co), C = the NHWC output, the bias one per column.  1 x 1 kernels with unit strides
-// and no padding: A is the images read in place as [n * H * W][C].  Chunks of whole images under LASER_B200_BATCH_WS_MB, the
-// tile count of each in int32, one preparation and one GEMM launch sequence each.
+// and no padding: A is the images read in place as [n * H * W][C].  Chunks of whole images (conv_nhwc_chunks).
 int conv2d_nhwc_fused_dev(float *output, const float *input, const ConvGeom &g, const float *kernel, const int64_t kernelStrides[2],
                           const laser_b200_epilogue *epi_in, int path, void *stream) {
   Epilogue epi;
@@ -1406,9 +1447,8 @@ int conv2d_nhwc_fused_dev(float *output, const float *input, const ConvGeom &g, 
     return set_error(LASER_B200_EINVAL, "a convolution's bias is one per output channel: bias_per_row must be 1");
   if (g.B == 0) return LASER_B200_OK;
   if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
-  const int64_t N = g.Cout, K = g.K(), P = g.outHW();
   if (path == LASER_B200_PATH_AUTO) path = conv_auto_path(g, epi);
-  if (is_tc_mode(path) && P > 0x7fffffffLL / g.B)
+  if (is_tc_mode(path) && g.outHW() > 0x7fffffffLL / g.B)
     return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: images * outH * outW must fit in int32");
   epi.bias_per_row = 0;   // the output channels are the columns of C
   const bool in_place = g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0;
@@ -1417,20 +1457,9 @@ int conv2d_nhwc_fused_dev(float *output, const float *input, const ConvGeom &g, 
   Ctx *c;
   if ((rc = get_ctx(&c))) return rc;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  const int64_t per = batch_ws_per_problem(path, P, N, K, true, false, !in_place, false);
-  int64_t chunk = per > 0 ? c->batch_ws_bytes / per : g.B;
-  const int64_t max_m_blocks = 0x7fffffffLL / (16 * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N));
-  if (chunk > max_m_blocks * TC_BLOCK_M / P) chunk = max_m_blocks * TC_BLOCK_M / P;
-  if (chunk < 1) chunk = 1;
-  const int64_t image = g.H * g.W * g.C;
-  for (int64_t b0 = 0; b0 < g.B; b0 += chunk) {
-    const int64_t imgs = g.B - b0 < chunk ? g.B - b0 : chunk;
-    gn.B = imgs;
-    if ((rc = run_f32(*c, path, imgs * P, N, K, 1.0f, input + b0 * image, g.C, 1, kernel, kernelStrides[0], kernelStrides[1], 0.0f,
-                      output + b0 * P * N, N, 1, s, epi, nullptr, nullptr, 0, nullptr, false, nullptr, nullptr,
-                      in_place ? nullptr : &gn)))
-      return rc;
-  }
+  if ((rc = conv_nhwc_chunks(*c, path, gn, g.Cout, 1.0f, input, kernel, kernelStrides[0], kernelStrides[1], 0.0f, output, s, epi,
+                             nullptr, in_place)))
+    return rc;
   g_last_path = path;
   return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
@@ -1475,7 +1504,8 @@ int conv2d_input_grad_dev(float *grad_input, const ConvGeom &g, const float *gra
   if ((rc = get_ctx(&c))) return rc;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
   // W' once per call into library workspace, K-major rows 16 bytes apart, read in place by every chunk's product.  The buffer
-  // is this entry's alone, held for the whole call; the copy waits for the last kernel that read it (ws_free).
+  // (tfilt, shared with the channels-last input gradient) is held for the whole call; the copy waits for the last kernel that
+  // read it (ws_free).
   std::lock_guard<std::mutex> lk(c->tfilt_mu);
   const int64_t lda = round_up(K, 4);
   if ((rc = ensure(c->tfilt, static_cast<size_t>(g.C * lda) * sizeof(float)))) return rc;
@@ -1486,6 +1516,67 @@ int conv2d_input_grad_dev(float *grad_input, const ConvGeom &g, const float *gra
   float *wt = static_cast<float *>(c->tfilt.ptr);
   if ((rc = launch_copy<uint32_t>(*c, wt, kernel + khw - 1, cp, s))) return rc;
   return conv_windows_dev(gt, alpha, wt, lda, 1, grad_output, beta, grad_input, opB, Epilogue(), path, stream);
+}
+
+// laser_b200_conv2d_nhwc_input_grad_f32_fused_dev (capi_layers.inc checks the geometry): NHWC output gradients and input
+// gradient, ONE product for the images of a chunk,
+//   dX[n * H * W + q][ci] <- alpha * sum_k' R[n * H * W + q][k'] * W'^T[ci][k'] + beta * dX[n * H * W + q][ci]
+// with k' = (kh' * kW + kw') * Cout + co, T = kH * kW, W'^T[ci][k'] = Wmat[(T - 1 - (kh' * kW + kw')) * C + ci][co]: M = n * H * W,
+// N = C, K' = T * Cout.  A = R, the input pixels' windows over op(dY) zero-dilated by the forward strides -- the transposed
+// geometry of conv2d_input_grad_dev, channels-last (split.cuh: Im2colNhwcGradSrc); B = W'^T, copied once per call into tfilt as
+// K-major rows [C][round_up(K', 4)]: no rank-2 view of the caller's filters has k' in (tap, co) order, and ordering A by (co,
+// tap) instead would lose its channel-contiguous loads.  1 x 1 kernels with unit strides and no padding: the plain product
+// op(dY) * Wmat^T, dY read in place as [n * P][Cout] and Wmat through its strides, no copy.  Chunks of whole images
+// (conv_nhwc_chunks).  PATH_AUTO: the path of conv2d_input_grad_dev for the same geometry.
+int conv2d_nhwc_input_grad_dev(float *grad_input, const ConvGeom &g, const float *grad_output, const float *kernel,
+                               const int64_t kernelStrides[2], float alpha, float beta, const laser_b200_operand_op *op_in, int path,
+                               void *stream) {
+  int rc;
+  if ((rc = check_f32_path(path))) return rc;
+  if (!kernelStrides) return set_error(LASER_B200_EINVAL, "kernelStrides is NULL");
+  OperandOp op;
+  const OperandOp *opA;
+  if ((rc = operand_op_of(op_in, false, &op, &opA))) return rc;
+  const int64_t khw = g.kH * g.kW;
+  if (opA && opA->aux && (opA->aux_sr != g.Cout || opA->aux_sc != 1))
+    return set_error(LASER_B200_EINVAL, "the aux tensor of op %d must be dense NHWC like grad_output: strides (%lld, 1), not (%lld, %lld)",
+                     opA->op, (long long)g.Cout, (long long)opA->aux_sr, (long long)opA->aux_sc);
+  if (g.B == 0) return LASER_B200_OK;
+  if (!grad_input || !grad_output || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
+  if (g.Cout > INT32_MAX / khw) return set_error(LASER_B200_EUNSUPPORTED, "c_out * kH * kW beyond 2^31");
+  ConvGeom gt = g;
+  gt.C = g.Cout; gt.H = g.outH; gt.W = g.outW; gt.Cout = g.C;
+  gt.pH = g.kH - 1 - g.pH; gt.pW = g.kW - 1 - g.pW;
+  gt.sH = gt.sW = 1;
+  gt.dH = g.sH; gt.dW = g.sW;
+  gt.outH = g.H; gt.outW = g.W;
+  gt.nhwc = true;
+  if (path == LASER_B200_PATH_AUTO) path = conv_auto_path(gt, Epilogue());
+  if (is_tc_mode(path) && gt.outHW() > 0x7fffffffLL / g.B)
+    return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: images * H * W must fit in int32");
+  const int64_t K = gt.K(), ks0 = kernelStrides[0], ks1 = kernelStrides[1];
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  if (khw == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0) {
+    rc = conv_nhwc_chunks(*c, path, gt, g.C, alpha, grad_output, kernel, ks1, ks0, beta, grad_input, s, Epilogue(), opA, true);
+  } else {
+    // W'^T once per call into tfilt (held for the whole call), K-major rows 16 bytes apart, read in place by every chunk's
+    // product; the copy waits for the last kernel that read the buffer (ws_free)
+    std::lock_guard<std::mutex> lk(c->tfilt_mu);
+    const int64_t lda = round_up(K, 4);
+    if ((rc = ensure(c->tfilt, static_cast<size_t>(g.C * lda) * sizeof(float)))) return rc;
+    CUDA_TRY(cudaStreamWaitEvent(s, c->ws_free, 0));
+    const int64_t shape[3] = {g.C, khw, g.Cout}, dst_st[3] = {lda, g.Cout, 1}, src_st[3] = {ks0, -g.C * ks0, ks1};
+    CopyParams cp;
+    copy_plan(3, shape, dst_st, src_st, &cp);
+    float *wt = static_cast<float *>(c->tfilt.ptr);
+    if ((rc = launch_copy<uint32_t>(*c, wt, kernel + (khw - 1) * g.C * ks0, cp, s))) return rc;
+    rc = conv_nhwc_chunks(*c, path, gt, g.C, alpha, grad_output, wt, 1, lda, beta, grad_input, s, Epilogue(), opA, false);
+  }
+  if (rc) return rc;
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -2095,5 +2186,6 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 #define LB200_CONV2D_FILTER_GRAD_F32 conv2d_filter_grad_dev
 #define LB200_CONV2D_NHWC_FILTER_GRAD_F32 conv2d_nhwc_filter_grad_dev
 #define LB200_CONV2D_INPUT_GRAD_F32 conv2d_input_grad_dev
+#define LB200_CONV2D_NHWC_INPUT_GRAD_F32 conv2d_nhwc_input_grad_dev
 #include "capi_layers.inc"
 #include "capi_multi.inc"

@@ -613,9 +613,74 @@ __device__ __forceinline__ float4 nhwc_window_vec(const float *__restrict__ img,
   return make_float4(v[0], v[1], v[2], v[3]);
 }
 
+// ---- channels-last transposed source: A of the NHWC input gradient, prepared straight from the NHWC output gradients ------
+// Row n * outHW + p -- input pixel p = ih * W + iw of image n -- is the pixel's window over dY zero-dilated by the forward
+// strides, in the order k' = (kh' * kW + kw') * c_out + co: the transposed geometry of Im2colGradSrc (C = c_out, H x W = outH x
+// outW, pH = kH - 1 - pH, stride 1, outW = the input's W), laid out like Im2colNhwcSrc's windows,
+//   row[k'] = op(dY)[n][h / dH][w / dW][co],  h = ih - pH' + kh', w = iw - pW' + kw'  when both are source positions, else 0
+// (holes are 0, never op(0); the aux at the same NHWC offset as the dY element).  vec (c_out % 4 == 0, dY and the aux 16-byte
+// aligned): every float4 of a row lies inside one tap, so the hole test and the h / dH decode run once per float4 and a
+// source value is one 16-byte load (and one of the aux).  A parameter struct of its own, so that Im2colNhwcSrc keeps its
+// layout.
+struct Im2colNhwcGradSrc : Im2colNhwcSrc {
+  int dH, dW;     // source dilation: the forward strides (1: none)
+  OperandOp op;   // HAS_OP: the op on the source values
+};
+// (h, w) of the dilated plane -> the source pixel, and whether there is one
+template <bool DIL>
+__device__ __forceinline__ bool dilated_source(const Im2colNhwcGradSrc &q, int &h, int &w) {
+  if constexpr (DIL) {   // h >= 0 is tested, and the quotient used, before any remainder of a negative h could matter
+    const unsigned hq = static_cast<unsigned>(h) / static_cast<unsigned>(q.dH), wq = static_cast<unsigned>(w) / static_cast<unsigned>(q.dW);
+    const bool inside = h >= 0 && w >= 0 && hq * q.dH == static_cast<unsigned>(h) && wq * q.dW == static_cast<unsigned>(w) &&
+                        hq < static_cast<unsigned>(q.H) && wq < static_cast<unsigned>(q.W);
+    h = static_cast<int>(hq);
+    w = static_cast<int>(wq);
+    return inside;
+  } else {
+    return static_cast<unsigned>(h) < static_cast<unsigned>(q.H) && static_cast<unsigned>(w) < static_cast<unsigned>(q.W);
+  }
+}
+// elements k .. k+3 of the channels-last transposed window of input pixel (oh, ow) of image `img` (aux: its aux image, HAS_OP)
+template <bool DIL, bool HAS_OP>
+__device__ __forceinline__ float4 nhwc_grad_window_vec(const float *__restrict__ img, const float *__restrict__ aux,
+                                                       const Im2colNhwcGradSrc &q, int oh, int ow, int k) {
+  const int tap = k / q.C;
+  int co = k - tap * q.C;
+  int kr = tap / q.kW, kc = tap - kr * q.kW;
+  if (q.vec) {   // k % 4 == 0 and c_out % 4 == 0: k .. k+3 are channels co .. co+3 of one tap
+    int h = oh - q.pH + kr, w = ow - q.pW + kc;
+    if (k < q.K && dilated_source<DIL>(q, h, w)) {
+      const int64_t off = (static_cast<int64_t>(h) * q.W + w) * q.C + co;
+      float4 v = *reinterpret_cast<const float4 *>(img + off);
+      if constexpr (HAS_OP) {
+        const float4 y = aux ? *reinterpret_cast<const float4 *>(aux + off) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        v = make_float4(operand_op(q.op.op, v.x, y.x), operand_op(q.op.op, v.y, y.y), operand_op(q.op.op, v.z, y.z),
+                        operand_op(q.op.op, v.w, y.w));
+      }
+      return v;
+    }
+    return make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  }
+  float v[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    int h = oh - q.pH + kr, w = ow - q.pW + kc;
+    float x = 0.0f;
+    if (k + e < q.K && dilated_source<DIL>(q, h, w)) {
+      const int64_t off = (static_cast<int64_t>(h) * q.W + w) * q.C + co;
+      x = img[off];
+      if constexpr (HAS_OP) x = operand_op(q.op.op, x, aux ? aux[off] : 0.0f);
+    }
+    v[e] = x;
+    if (++co == q.C) { co = 0; if (++kc == q.kW) { kc = 0; ++kr; } }
+  }
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+
 template <bool GRAD, bool NHWC = false>
-using Im2colSrcOf =
-    typename std::conditional<NHWC, Im2colNhwcSrc, typename std::conditional<GRAD, Im2colGradSrc, Im2colSrc>::type>::type;
+using Im2colSrcOf = typename std::conditional<
+    NHWC, typename std::conditional<GRAD, Im2colNhwcGradSrc, Im2colNhwcSrc>::type,
+    typename std::conditional<GRAD, Im2colGradSrc, Im2colSrc>::type>::type;
 // elements k .. k+3 of the transposed window of pixel (oh, ow) of image `img` (aux: its aux image, HAS_OP)
 template <bool DIL, bool HAS_OP>
 __device__ __forceinline__ float4 grad_window_vec(const float *__restrict__ img, const float *__restrict__ aux, const Im2colGradSrc &q,
@@ -652,21 +717,22 @@ __device__ __forceinline__ float4 grad_window_vec(const float *__restrict__ img,
 template <bool DIL, bool HAS_OP, bool NHWC, typename Src>
 __device__ __forceinline__ float4 source_vec(const float *__restrict__ img, const float *__restrict__ aux, const Src &q, int oh, int ow,
                                              int k) {
-  if constexpr (NHWC) return nhwc_window_vec(img, q, oh, ow, k);
+  if constexpr (NHWC && (DIL || HAS_OP)) return nhwc_grad_window_vec<DIL, HAS_OP>(img, aux, q, oh, ow, k);
+  else if constexpr (NHWC) return nhwc_window_vec(img, q, oh, ow, k);
   else if constexpr (DIL || HAS_OP) return grad_window_vec<DIL, HAS_OP>(img, aux, q, oh, ow, k);
   else return window_vec(img, q, oh, ow, k);
 }
 
 // (F16X2: the row in registers next to the geometry needs more than the 64 registers of 4 CTAs per SM -- it spills there)
 // DIL / HAS_OP (an Im2colGradSrc): the transposed source of the input gradient, dilated / with an op; NHWC (an Im2colNhwcSrc):
-// the channels-last source of the NHWC forward call; the NCHW forward call's instantiations are <MODE, GROUP, false, false>.
+// the channels-last source of the NHWC forward call, with DIL / HAS_OP (an Im2colNhwcGradSrc) the channels-last transposed
+// source of the NHWC input gradient; the NCHW forward call's instantiations are <MODE, GROUP, false, false>.
 template <int MODE, int GROUP, bool DIL = false, bool HAS_OP = false, bool NHWC = false>
 __global__ void __launch_bounds__(256, MODE == IM2COL_F16X2 ? 3 : 4)
 im2col_rows_kernel(const float *__restrict__ in, Im2colSrcOf<DIL || HAS_OP, NHWC> q, int64_t images, float *__restrict__ dst,
                    float *__restrict__ dst_lo, uint16_t *__restrict__ hb, uint16_t *__restrict__ lb, int64_t ld,
                    uint32_t *__restrict__ absmax) {
   static_assert(GROUP == 32 || GROUP == 256, "a warp or the CTA per row");
-  static_assert(!NHWC || !(DIL || HAS_OP), "the channels-last source has no dilation or op");
   __shared__ uint32_t red[2][8];
   ptx::griddep_launch_dependents();   // the next kernel of the stream may start its prologue (it waits for our results)
   const int tid = static_cast<int>(threadIdx.x) % GROUP;

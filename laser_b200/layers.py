@@ -15,6 +15,8 @@
                                                   tap rows transposed out of the images in the operand preparation
     conv2d_input_grad_fused                       its input gradient, the transposed window gather over grad_output folded
                                                   into the operand preparation
+    conv2d_nhwc_input_grad_fused                  the input gradient of conv2d_nhwc_fused: NHWC gradients, the transposed
+                                                  windows gathered along the channels in the operand preparation
     gemm_strided_batched                          (roadmap item of the reference, README.md:253-263)
     copyFrom(dst, src)                            laser/tensor/initialization.nim:80-112
 
@@ -246,6 +248,32 @@ def conv2d_input_grad_fused(grad_input, ishape, grad_output, kernel, kshape, pad
     check(lib().laser_b200_conv2d_input_grad_f32_fused_dev(pg, _i4(ishape), po, pk, _i4(kshape), _i2(padding), _i2(strides),
                                                            float(alpha), float(beta), ctypes.byref(o) if o is not None else None,
                                                            int(path), stream))
+
+
+def conv2d_nhwc_input_grad_fused(grad_input, ishape, grad_output, kernel, kshape, padding, strides, alpha=1.0, beta=0.0, op=None,
+                                 aux=None, path=PATH_AUTO, stream=None, kernel_strides=None):
+    """grad_input <- alpha * conv_transpose(op(grad_output), kernel) + beta * grad_input on float32 DEVICE buffers: the input
+    gradient of conv2d_nhwc_fused (grad_input dense NHWC [n, h, w, c_in], grad_output dense NHWC [n, outH, outW, c_out]).
+    kernel: the 2-D device view [kH * kW * c_in, c_out] of the filter matrix conv2d_nhwc_fused takes, its element strides read
+    from the view (kernel_strides: for a pointer without strides).  op and aux as for conv2d_nhwc_filter_grad_fused, applied
+    to grad_output.  beta=1 accumulates into an existing gradient.  One product for the images, its A operand (the windows
+    over grad_output, zero-dilated by the strides) prepared straight from grad_output: no conversion to NCHW."""
+    pg, po, pk = _dev_f32(grad_input), _dev_f32(grad_output), _dev_f32(kernel)
+    if kernel_strides is None:
+        kernel_strides = tuple(kernel.stride())
+    if len(kernel_strides) != 2:
+        raise ValueError("kernel must be a 2-D view [kH * kW * c_in, c_out]")
+    o = None
+    if op is not None:
+        o = OperandOp()
+        o.op = OP_NAMES[op]
+        if aux is not None:
+            o.aux = _dev_f32(aux)
+            o.auxRowStride, o.auxColStride = kshape[0], 1
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_nhwc_input_grad_f32_fused_dev(pg, _i4(ishape), po, pk, _i4(kshape), _i2(kernel_strides),
+                                                                _i2(padding), _i2(strides), float(alpha), float(beta),
+                                                                ctypes.byref(o) if o is not None else None, int(path), stream))
 
 
 def gemm_strided_batched(batch, M, N, K, alpha, A, rowStrideA, colStrideA, batchStrideA, B, rowStrideB, colStrideB,
