@@ -453,6 +453,35 @@ int laser_b200_conv2d_im2col_f32_dev(float *output, const float *input, const in
 int laser_b200_conv2d_f32_fused_dev(float *output, const float *input, const int64_t ishape[4],
                                     const float *kernel, const int64_t kshape[4], const int64_t padding[2],
                                     const int64_t strides[2], const laser_b200_epilogue *epi, int path, void *stream);
+/* Grouped fused convolution (torch.nn.Conv2d(groups=G); the reference has no grouped layers): for every image n and group g,
+ *   output_n[g * Mg .. (g + 1) * Mg) <- act(conv(input_n[g * Cg .. (g + 1) * Cg), kernel[g * Mg .. (g + 1) * Mg)) + bias)
+ * with Cg = c_in / groups, Mg = c_out / groups, ishape = (n, c_in, h, w) and kshape = (c_out, c_in / groups, kH, kW) (torch's
+ * grouped weight).  input, kernel and output are dense NCHW / [c_out][c_in / groups][kH][kW] / NCHW device buffers; the
+ * output is fully overwritten (alpha 1, beta 0).  In im2col terms, with Kg = Cg * kH * kW and co = g * Mg + m:
+ *   output[n][co] = act(sum_{k < Kg} kernel[co][k] * im2col(input[n][g * Cg .. (g + 1) * Cg))[k] + bias[co]),
+ * k = ci * kH * kW + kh * kW + kw as in the forward call.
+ *   epi: bias_per_row = 1 is one bias per output channel (a bias with bias_per_row = 0 is EINVAL); NULL epi = no bias, no
+ *   activation.
+ *   groups == 1 is laser_b200_conv2d_f32_fused_dev: the same bits, launches and last_path on every path.
+ *   PATH_SIMT (exact): a direct convolution on the CUDA cores, ONE launch for every image and group, no workspace.  Each output
+ *   is the exact GEMM's fmaf chain over its group's im2col column (restarted every 512 k-steps, the blocks added in order),
+ *   and bias and activation are the exact kernel's, so the output is bit for bit the oracle's conv2d_im2col of each group's
+ *   slice; taps in the padding are multiplied by zero, so an Inf or NaN filter tap there gives NaN as in that GEMM.
+ *   Tensor-core paths: the n * G per-group problems -- image n's channel slice of group g -- are ONE batched GEMM per chunk of
+ *   whole images (LASER_B200_BATCH_WS_MB), whose A is the filters prepared once as G problems of Mg x Kg, problem n * G + g
+ *   reading group g's filters and bias: 3 launches per chunk (filter rows, window rows, GEMM; split-K adds a reduce).  For
+ *   Kg <= 768 the bits equal G calls of conv2d_f32_fused_dev on contiguous per-group copies on the same path.
+ *   PATH_AUTO: conv2d_f32_fused_dev's decision for the per-group geometry (n * G images of Cg channels, c_out = Mg): the exact
+ *   path when Mg < 64 or Kg < 64 (every depthwise layer), else the tensor-core path of one group.
+ *   n = 0: LASER_B200_OK, nothing launched, output untouched.
+ *   LASER_B200_EINVAL, before anything is launched: groups < 1; c_in or c_out not a multiple of groups; kshape[1] * groups !=
+ *   c_in; geometry errors; an unknown path or activation; the bias rule above; a NULL pointer.
+ *   LASER_B200_EUNSUPPORTED: on a tensor-core path, when n * G problems (one chunk's at least) or their tiles do not fit in
+ *   int32; on the exact path, a kernel window too large for the direct kernel's shared-memory tile (thousands of taps). */
+int laser_b200_conv2d_grouped_f32_fused_dev(float *output, const float *input, const int64_t ishape[4],
+                                            const float *kernel, const int64_t kshape[4], const int64_t padding[2],
+                                            const int64_t strides[2], int64_t groups, const laser_b200_epilogue *epi,
+                                            int path, void *stream);
 /* Channels-last fused convolution (conv2d_mec's NHWC layout and [kH][kW][C_in][C_out] filters, benchmarks/convolution/
  * conv2d_mec.nim, with padding): for every image n,
  *   output_n <- act(conv(input_n, kernel) + bias)

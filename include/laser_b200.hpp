@@ -17,6 +17,7 @@
 //   laser::TensorShape/KernelShape/Padding/Strides, conv2d_out_shape, im2col_workspace_size,
 //   conv2d_im2col                                     benchmarks/convolution/conv2d_common.nim:6-45,
 //                                                     conv2d_im2col.nim:8-166
+//   laser::conv2d_grouped_fused_dev                   torch.nn.Conv2d(groups=G) on device buffers
 #pragma once
 
 #include <cstdint>
@@ -244,6 +245,15 @@ inline void conv2d_im2col(float *output, TensorShape oshape, const float *input,
   const int64_t is[4] = {ishape.n, ishape.c, ishape.h, ishape.w}, ks[4] = {kshape.c_out, kshape.c_in, kshape.kH, kshape.kW};
   const int64_t pd[2] = {padding.h, padding.w}, st[2] = {strides.h, strides.w};
   check(laser_b200_conv2d_im2col_f32(output, input, is, kernel, ks, pd, st));
+}
+// grouped fused convolution on device buffers (laser_b200_conv2d_grouped_f32_fused_dev): kernel (c_out, c_in / groups, kH, kW),
+// epi NULL = no bias, no activation; stream NULL = the library's stream, synchronous
+inline void conv2d_grouped_fused_dev(float *output, const float *input, TensorShape ishape, const float *kernel, KernelShape kshape,
+                                     Padding padding, Strides strides, int64_t groups, const laser_b200_epilogue *epi = nullptr,
+                                     int path = LASER_B200_PATH_AUTO, void *stream = nullptr) {
+  const int64_t is[4] = {ishape.n, ishape.c, ishape.h, ishape.w}, ks[4] = {kshape.c_out, kshape.c_in, kshape.kH, kshape.kW};
+  const int64_t pd[2] = {padding.h, padding.w}, st[2] = {strides.h, strides.w};
+  check(laser_b200_conv2d_grouped_f32_fused_dev(output, input, is, kernel, ks, pd, st, groups, epi, path, stream));
 }
 
 }  // namespace laser

@@ -128,6 +128,8 @@ SIGNATURES = {
     "laser_b200_conv2d_im2col_f32": (ctypes.c_int, [vp, vp, i64 * 4, vp, i64 * 4, i64 * 2, i64 * 2]),
     "laser_b200_conv2d_f32_fused_dev": (ctypes.c_int, [vp, vp, i64 * 4, vp, i64 * 4, i64 * 2, i64 * 2, ctypes.POINTER(Epilogue),
                                                        ctypes.c_int, vp]),
+    "laser_b200_conv2d_grouped_f32_fused_dev": (ctypes.c_int, [vp, vp, i64 * 4, vp, i64 * 4, i64 * 2, i64 * 2, i64,
+                                                               ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
     "laser_b200_conv2d_nhwc_f32_fused_dev": (ctypes.c_int, [vp, vp, i64 * 4, vp, i64 * 4, i64 * 2, i64 * 2, i64 * 2,
                                                             ctypes.POINTER(Epilogue), ctypes.c_int, vp]),
     "laser_b200_conv2d_filter_grad_f32_fused_dev": (ctypes.c_int, [vp, vp, i64 * 4, vp, i64 * 4, i64 * 2, i64 * 2, f32, f32,

@@ -788,18 +788,19 @@ inline TcKind tc_kind_of_path(int path) {
 }
 inline SplitMode split_mode(TcKind k) { return k == TC_TF32X3 ? SPLIT_TF32 : k == TC_F16X3 ? SPLIT_F16X2 : SPLIT_NONE; }
 
-// a batched launch: `batch` problems, C of problem b at C + b * C_stride
+// a batched launch: `batch` problems, C of problem b at C + b * C_stride; a per-row bias of problem b at bias + (b % A's period)
+// * bias_stride (0: one bias for the batch)
 struct BatchArgs {
-  int64_t batch, C;
+  int64_t batch, C, bias = 0;
 };
 
 // launch the tensor-core kernel on prepared operands (c.mu held by the caller).  bat: a batched launch (tc_params.h; the maps
-// are rank 3), with a_shared / b_shared for operands prepared once for the whole batch.
+// are rank 3), problem b reading slice b % period_a of A and b % period_b of B (1: an operand prepared once for the batch).
 template <typename OutT>
 int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, const OperandMaps &ma,
            const OperandMaps &mb, float beta, OutT *C, int64_t rsC, int64_t csC, cudaStream_t s,
            const Epilogue &epi, const F16Scales *f16 = nullptr, bool after_prep = false, const BatchArgs *bat = nullptr,
-           bool a_shared = false, bool b_shared = false) {
+           int64_t period_a = 1, int64_t period_b = 1) {
   TcLaunch l;
   l.a0 = ma.p0; l.a1 = ma.p1; l.b0 = mb.p0; l.b1 = mb.p1;
   l.a_mn = ma.mn_major; l.b_mn = mb.mn_major;
@@ -812,11 +813,12 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
   if (bat) {
     l.batched = true;
     p.batch = static_cast<int>(bat->batch);
-    p.map_b_a = a_shared ? 0 : 1;
-    p.map_b_b = b_shared ? 0 : 1;
+    p.period_a = static_cast<int>(period_a);
+    p.period_b = static_cast<int>(period_b);
     p.bsC = bat->C;
-    p.amax_bs_a = a_shared ? 0 : M;
-    p.amax_bs_b = b_shared ? 0 : N;
+    p.amax_bs_a = M;
+    p.amax_bs_b = N;
+    p.bias_bs = bat->bias;
   }
   const int npass = (kind == TC_TF32X3 || kind == TC_F16X3) ? 3 : 1;
   const TcPlanCfg cfg{c.kc_faithful, c.raster_g, c.splitk_enabled, c.sm_count};
@@ -859,7 +861,7 @@ int tc_run(Ctx &c, TcKind kind, int64_t M, int64_t N, int64_t K, float alpha, co
       auto reduce = [&](auto batched) {
         splitk_tail_reduce_kernel<decltype(batched)::value><<<grid_for(c, items, 8), 256, 0, s>>>(
             static_cast<const float *>(c.splitk.ptr), p.k_splits, n_tail, p.n_direct, p.num_m_blocks, p.num_n_blocks, p.raster_g,
-            M, N, alpha, beta, C, rsC, csC, p.epi.bias, p.epi.bias_per_row, p.epi.act, p.bsC);
+            M, N, alpha, beta, C, rsC, csC, p.epi.bias, p.epi.bias_per_row, p.epi.act, p.bsC, p.period_a, p.bias_bs);
       };
       if (bat) reduce(std::true_type());
       else reduce(std::false_type());
@@ -887,8 +889,9 @@ int gemm_tc(Ctx &c, TcKind kind, const Operand &oa, const Operand &ob, float alp
   // b_ready: B becomes valid only when this event has fired (the row-sharded driver: B is in flight on the communication
   // stream); everything that does not read B -- the preparation of A -- is queued before the wait.
   // opA / opB: operand ops applied while the operands are prepared (fp32 only)
-  // bat: a batched launch, every problem's operand in the same launches.  Concatenated operands (Operand::concat): one
-  // product of extent batch * K (one problem for the GEMM: rank-2 maps, one scale word per row of A and column of B).
+  // bat: a batched launch, every problem's operand in the same launches; an operand of batch_of(o).n < bat->batch problems
+  // repeats with that period.  Concatenated operands (Operand::concat): one product of extent batch * K (one problem for the
+  // GEMM: rank-2 maps, one scale word per row of A and column of B).
   const int64_t M = oa.mn, N = ob.mn, K = oa.k;
   const bool cat = oa.concat;
   const int64_t Kt = cat ? batch_of(oa).n * K : K;   // (the entry bounds batch * K by INT64_MAX)
@@ -896,7 +899,6 @@ int gemm_tc(Ctx &c, TcKind kind, const Operand &oa, const Operand &ob, float alp
     return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: extents must fit in int32");
   std::lock_guard<std::mutex> lk(c.mu);  // workspace + descriptor construction are per context
   const SplitMode mode = split_mode(kind);
-  const bool a_shared = bat && batch_shares(oa.s_b, opA, oa.aux_sb), b_shared = bat && batch_shares(ob.s_b, opB, ob.aux_sb);
   OperandMaps ma, mb;
   bool used_ws = false;
   // the previous call may still be reading the workspace on another stream
@@ -916,7 +918,7 @@ int gemm_tc(Ctx &c, TcKind kind, const Operand &oa, const Operand &ob, float alp
   const F16Scales f16{static_cast<const uint32_t *>(c.f16s.ptr), static_cast<const uint32_t *>(c.f16s.ptr) + f16_b_off};
   // (with profiling on, an event record sits between the last preparation kernel and the GEMM: no dependent launch then)
   rc = tc_run<OutT>(c, kind, M, N, Kt, alpha, ma, mb, beta, C, rsC, csC, s, epi, mode == SPLIT_F16X2 ? &f16 : nullptr,
-                    prep_launches > 0 && !c.profiling, bat, a_shared, b_shared);
+                    prep_launches > 0 && !c.profiling, bat, batch_of(oa).n, batch_of(ob).n);
   if (rc) return rc;
   if (used_ws) CUDA_TRY(cudaEventRecord(c.ws_free, s));
   return LASER_B200_OK;
@@ -1121,21 +1123,26 @@ int simt_run(Ctx &c, const Operand &oa, const Operand &ob, float alpha, float be
 //     (ConvGeom::taps): N = the taps, K = images * outH * outW pixels of the images at B (a single problem).
 //   convA: A is a channels-last im2col source (ConvGeom::nhwc), M = images * outH * outW rows of the images at A (rsA, csA
 //     unused; a single problem).
+//   periodA > 0 (batched, tensor cores): A is periodA problems bs->A apart and problem b reads A_{b % periodA} -- the filters of
+//     a grouped convolution --, a per-row bias periodA blocks of M, problem b reading block b % periodA.
 int run_f32(Ctx &c, int path, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA, const float *B,
             int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC, cudaStream_t s, const Epilogue &epi,
             const OperandOp *opA, const OperandOp *opB, int64_t batch = 0, const laser_b200_batch_strides *bs = nullptr,
-            bool concat = false, const ConvGeom *convB = nullptr, cudaEvent_t b_ready = nullptr, const ConvGeom *convA = nullptr) {
+            bool concat = false, const ConvGeom *convB = nullptr, cudaEvent_t b_ready = nullptr, const ConvGeom *convA = nullptr,
+            int64_t periodA = 0) {
   Operand oa{A, M, K, rsA, csA}, ob{B, N, K, csB, rsB};
   if (batch > 0) {
-    oa.batch = !concat && batch_shares(bs->A, opA, bs->auxA) ? 1 : batch; oa.s_b = bs->A; oa.aux_sb = bs->auxA; oa.concat = concat;
+    oa.batch = periodA > 0 ? periodA : !concat && batch_shares(bs->A, opA, bs->auxA) ? 1 : batch; oa.s_b = bs->A; oa.aux_sb = bs->auxA; oa.concat = concat;
     ob.batch = !concat && batch_shares(bs->B, opB, bs->auxB) ? 1 : batch; ob.s_b = bs->B; ob.aux_sb = bs->auxB; ob.concat = concat;
   }
   oa.conv = convA;
   ob.conv = convB;
   const bool batched = batch > 0 && !concat;
+  if (periodA > 0 && (!batched || opA || path == LASER_B200_PATH_SIMT))
+    return set_error(LASER_B200_ECUDA, "internal: a periodic A is a batched tensor-core operand without op");
   if (path == LASER_B200_PATH_SIMT)
     return simt_run(c, oa, ob, alpha, beta, C, rsC, csC, s, epi, opA, opB, batched ? batch : 1, batched ? bs->C : 0);
-  const BatchArgs bat{batch, batched ? bs->C : 0};
+  const BatchArgs bat{batch, batched ? bs->C : 0, periodA > 0 ? M : 0};
   return gemm_tc<4, float>(c, tc_kind_of_path(path), oa, ob, alpha, beta, C, rsC, csC, s, epi, b_ready, opA, opB,
                            batched ? &bat : nullptr);
 }
@@ -1282,11 +1289,12 @@ int64_t batch_ws_per_problem(int path, int64_t M, int64_t N, int64_t K, bool a_o
   return (a_own ? one(M, opA) : 0) + (b_own ? one(N, opB) : 0);
 }
 
-// convB: B is an im2col source (a convolution, run_f32): even one image takes the batched launch
+// convB: B is an im2col source (a convolution, run_f32): even one image takes the batched launch.  periodA > 0: A and a
+// per-row bias repeat with that period (run_f32), every chunk a whole number of periods.
 int batched_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alpha, const float *A, int64_t rsA, int64_t csA,
                       const float *B, int64_t rsB, int64_t csB, float beta, float *C, int64_t rsC, int64_t csC,
                       const laser_b200_batch_strides *bs, const OperandOp *opA, const OperandOp *opB, const Epilogue &epi,
-                      int path, void *stream, const ConvGeom *convB = nullptr) {
+                      int path, void *stream, const ConvGeom *convB = nullptr, int64_t periodA = 0) {
   if (batch < 0) return set_error(LASER_B200_EINVAL, "negative batch %lld", (long long)batch);
   if (batch > 0 && !bs) return set_error(LASER_B200_EINVAL, "batchStrides is NULL");
   if (batch > 1 && bs->C == 0) return set_error(LASER_B200_EINVAL, "batchStrides->C is 0: the problems' outputs would overlap");
@@ -1303,18 +1311,28 @@ int batched_fused_dev(int64_t batch, int64_t M, int64_t N, int64_t K, float alph
   if (path == LASER_B200_PATH_AUTO) path = resolve_auto(M, N, K, epi, /*operand_op=*/true);
   // chunks of whole problems: the prepared workspace stays under the cap, and the launch's tile counts -- batch x tiles x
   // up to 16 K-splits -- fit in int32 (an im2col source counts as an op'd B: the exact path writes its rows)
-  const int64_t per = batch_ws_per_problem(path, M, N, K, !batch_shares(bs->A, opA, bs->auxA), !batch_shares(bs->B, opB, bs->auxB),
-                                           opA != nullptr, opB != nullptr || convB);
+  // (a periodic A is prepared once, its periodA slices are not workspace per problem)
+  const int64_t per = batch_ws_per_problem(path, M, N, K, periodA == 0 && !batch_shares(bs->A, opA, bs->auxA),
+                                           !batch_shares(bs->B, opB, bs->auxB), opA != nullptr, opB != nullptr || convB);
   int64_t chunk = per > 0 ? c->batch_ws_bytes / per : batch;
   const int64_t tiles = ((M + TC_BLOCK_M - 1) / TC_BLOCK_M) * ((N + TC_BLOCK_N - 1) / TC_BLOCK_N);
   if (chunk > 0x7fffffffLL / (16 * tiles)) chunk = 0x7fffffffLL / (16 * tiles);
+  if (periodA > 0) {
+    if (periodA > 0x7fffffffLL / (16 * tiles))
+      return set_error(LASER_B200_EUNSUPPORTED, "tensor-core path: %lld problems of %lld tiles do not fit in int32",
+                       (long long)periodA, (long long)tiles);
+    chunk -= chunk % periodA;
+    if (chunk < periodA) chunk = periodA;
+  }
   if (chunk < 1) chunk = 1;
   for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
     OperandOp ca, cb;
     if (opA) { ca = *opA; if (ca.aux) ca.aux += b0 * bs->auxA; }
     if (opB) { cb = *opB; if (cb.aux) cb.aux += b0 * bs->auxB; }
-    if ((rc = run_f32(*c, path, M, N, K, alpha, A + b0 * bs->A, rsA, csA, B + b0 * bs->B, rsB, csB, beta, C + b0 * bs->C, rsC, csC, s,
-                      epi, opA ? &ca : nullptr, opB ? &cb : nullptr, batch - b0 < chunk ? batch - b0 : chunk, bs, false, convB)))
+    // (a chunk of a periodic batch starts at a whole period: problem b0 reads A's first slice)
+    if ((rc = run_f32(*c, path, M, N, K, alpha, periodA > 0 ? A : A + b0 * bs->A, rsA, csA, B + b0 * bs->B, rsB, csB, beta,
+                      C + b0 * bs->C, rsC, csC, s, epi, opA ? &ca : nullptr, opB ? &cb : nullptr, batch - b0 < chunk ? batch - b0 : chunk,
+                      bs, false, convB, nullptr, nullptr, periodA)))
       return rc;
   }
   g_last_path = path;
@@ -1401,6 +1419,58 @@ int conv2d_fused_dev(float *output, const float *input, const ConvGeom &g, const
   if (g.B == 0) return LASER_B200_OK;
   if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
   return conv_windows_dev(g, 1.0f, kernel, g.K(), 1, input, 0.0f, output, nullptr, epi, path, stream);
+}
+
+// laser_b200_conv2d_grouped_f32_fused_dev (capi_layers.inc checks the geometry and the groups; groups == 1 never comes here):
+// G groups of Cg = C / G input and Mg = Cout / G output channels.  Per group, the per-group geometry gp -- n * G images of Cg
+// channels, Cout = Mg -- is a batch of convolutions whose problem b = i * G + g reads image i's channel slice of group g (one
+// image of gp, the NCHW slices are Cg * H * W apart), writes output channels g * Mg .. (one output image of gp) and reads the
+// filters and bias of group b % G.
+//   PATH_AUTO: conv_auto_path over gp.  The exact path is the direct kernel (gemm_simt.cuh: conv_grouped_direct_kernel), one launch; the tensor-core
+//   paths are the batched fused product over gp with A = the filters as G problems of Mg x Kg, periodic with period G
+//   (batched_fused_dev), in chunks of whole images.
+int conv2d_grouped_fused_dev(float *output, const float *input, const ConvGeom &g, int64_t groups, const float *kernel,
+                             const laser_b200_epilogue *epi_in, int path, void *stream) {
+  Epilogue epi;
+  int rc;
+  if ((rc = epilogue_of(epi_in, &epi))) return rc;
+  if ((rc = check_f32_path(path))) return rc;
+  if (epi.bias && !epi.bias_per_row)
+    return set_error(LASER_B200_EINVAL, "a convolution's bias is one per output channel: bias_per_row must be 1");
+  if (g.B == 0) return LASER_B200_OK;
+  if (!output || !input || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
+  ConvGeom gp = g;
+  gp.B = g.B * groups;
+  gp.C = g.C / groups;
+  gp.Cout = g.Cout / groups;
+  if (path == LASER_B200_PATH_AUTO) path = conv_auto_path(gp, epi);
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  if (path == LASER_B200_PATH_SIMT) {
+    ConvGroupedParams p;
+    int mc;
+    size_t smem;
+    const int threads = conv_grouped_plan(g, groups, epi.bias, epi.act, &p, &mc, &smem);
+    if (threads == 0)
+      return set_error(LASER_B200_EUNSUPPORTED, "grouped convolution: a %lld x %lld kernel window does not fit in shared memory",
+                       (long long)g.kH, (long long)g.kW);
+    const int grid = grid_for(*c, p.tiles, 2048 / threads);
+    if (mc == 4) conv_grouped_direct_kernel<4><<<grid, threads, smem, s>>>(output, input, kernel, p);
+    else if (mc == 2) conv_grouped_direct_kernel<2><<<grid, threads, smem, s>>>(output, input, kernel, p);
+    else conv_grouped_direct_kernel<1><<<grid, threads, smem, s>>>(output, input, kernel, p);
+    COUNT_LAUNCH();
+    CHECK_LAUNCH();
+  } else {
+    const int64_t M = gp.Cout, K = gp.K(), N = gp.outHW(), image = gp.C * gp.H * gp.W;
+    const bool in_place = g.kH * g.kW == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0;
+    const laser_b200_batch_strides bs{M * K, image, M * N, 0, 0};
+    if ((rc = batched_fused_dev(gp.B, M, N, K, 1.0f, kernel, K, 1, input, N, 1, 0.0f, output, N, 1, &bs, nullptr, nullptr, epi, path,
+                                s, in_place ? nullptr : &gp, groups)))
+      return rc;
+  }
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
 
 // The product of both channels-last convolution entries, over the NHWC images `src` (a geometry with nhwc set) at A:
@@ -2183,6 +2253,7 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 #define LB200_BATCHED_FUSED_F32 batched_fused_entry
 #define LB200_CONV2D_FUSED_F32 conv2d_fused_dev
 #define LB200_CONV2D_NHWC_FUSED_F32 conv2d_nhwc_fused_dev
+#define LB200_CONV2D_GROUPED_FUSED_F32 conv2d_grouped_fused_dev
 #define LB200_CONV2D_FILTER_GRAD_F32 conv2d_filter_grad_dev
 #define LB200_CONV2D_NHWC_FILTER_GRAD_F32 conv2d_nhwc_filter_grad_dev
 #define LB200_CONV2D_INPUT_GRAD_F32 conv2d_input_grad_dev

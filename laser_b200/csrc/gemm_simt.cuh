@@ -23,6 +23,7 @@
 
 #include <type_traits>
 
+#include "layers.cuh"
 #include "ptx.cuh"
 
 namespace lb200 {
@@ -495,5 +496,190 @@ gemm_skinny_m_async_kernel(const SimtParams<float> p) {
   ptx::cp_async_wait<0>();
 }
 template <int MT> constexpr size_t ska_smem_bytes() { return (static_cast<size_t>(SKA_STAGES) * SKA_K * 256 + SKINNY_KCHUNK * (MT / 4)) * sizeof(float4); }
+
+// ---------------------------------------------------------------------------
+// Direct grouped convolution: the exact path of laser_b200_conv2d_grouped_f32_fused_dev, a convolution on the CUDA cores,
+// one launch, no preparation pass and no workspace.
+//
+// NCHW images [n][C][H][W], filters [Cout][Cg][kH][kW] (torch's grouped weight), G groups of Cg = C / G input and
+// Mg = Cout / G output channels.  Output channel co = g * Mg + m of image i:
+//   out[i][co] = act(sum_{k < Kg} w[co][k] * im2col(in[i][g * Cg : (g + 1) * Cg])[k] + bias[co]),  Kg = Cg * kH * kW
+// Each output is the exact GEMM's chain over the im2col matrix of its group (gemm_simt_kernel.inc), so the path is bit for
+// bit the oracle's conv2d_im2col of each group's slice:
+//   - one fmaf chain from 0 over k = ci * kH * kW + kh * kW + kw, restarted every KC = 512 k-steps, the block sums added in
+//     order (v = 0 + acc_0, v = v + acc_1, ...: the alpha = 1, beta' = 0 then 1 epilogue of the exact kernel);
+//   - taps in the padding are fmaf(w, 0, acc), not skipped (the staged patch holds the zeros), so an Inf or NaN filter tap
+//     gives NaN wherever the GEMM over the im2col matrix does;
+//   - bias and activation through simt_bias_act, the exact kernel's function.
+//
+// A CTA computes a tile of one image and one group: CG * MC output channels x TY output rows x 4 * XT output columns.
+// Thread (cg, ty, tx) owns MC consecutive channels and the 4 pixels tx, tx + XT, tx + 2 XT, tx + 3 XT of row ty: the
+// lanes of a warp read consecutive patch words (no bank conflict at unit stride) and store consecutive output words.  For
+// each input channel ci of the group the CTA stages in shared memory the zero-padded input rows and columns the tile
+// reads, [PR][PC], and the tile's filter taps of ci, [kH * kW][CG * MC] (a thread's MC weights of one tap in one 4-, 8- or
+// 16-byte load); the FMAs then read only shared memory.  Depthwise layers (Cg = 1) stage one channel per CTA tile.
+// ---------------------------------------------------------------------------
+constexpr int CONV_GROUPED_PX = 4;                 // output pixels per thread, XT apart along a row
+constexpr int CONV_GROUPED_THREADS = 256;          // most threads of a CTA
+constexpr int CONV_GROUPED_SMEM = 48 * 1024;       // most shared memory of a CTA (no opt-in needed)
+
+struct ConvGroupedParams {
+  int64_t images;
+  int C, H, W, G, Cg, Mg, kH, kW, pH, pW, sH, sW, outH, outW;
+  int XT, TY, CG;                    // threads along a row, rows, channel groups of MC per CTA
+  int x_tiles, y_tiles, m_tiles;     // CTA tiles per image and group
+  int PR, PC;                        // staged patch: rows, columns
+  int64_t tiles;                     // images * G * m_tiles * y_tiles * x_tiles
+  const float *bias;
+  int act;
+};
+
+// Host side: the tile of a geometry (C, Cout, ... of the whole layer; G groups).  *mc = channels per thread (1, 2 or 4:
+// the largest that divides Mg).  Returns the threads of a CTA, or 0 when even a one-row, one-quad tile needs more than
+// CONV_GROUPED_SMEM bytes (a kernel window of thousands of taps).  *smem_bytes: the CTA's dynamic shared memory.
+inline int conv_grouped_plan(const ConvGeom &g, int64_t G, const float *bias, int act, ConvGroupedParams *p, int *mc,
+                             size_t *smem_bytes) {
+  p->images = g.B;
+  p->C = static_cast<int>(g.C); p->H = static_cast<int>(g.H); p->W = static_cast<int>(g.W);
+  p->G = static_cast<int>(G); p->Cg = static_cast<int>(g.C / G); p->Mg = static_cast<int>(g.Cout / G);
+  p->kH = static_cast<int>(g.kH); p->kW = static_cast<int>(g.kW); p->pH = static_cast<int>(g.pH); p->pW = static_cast<int>(g.pW);
+  p->sH = static_cast<int>(g.sH); p->sW = static_cast<int>(g.sW);
+  p->outH = static_cast<int>(g.outH); p->outW = static_cast<int>(g.outW);
+  p->bias = bias;
+  p->act = act;
+  *mc = p->Mg % 4 == 0 ? 4 : p->Mg % 2 == 0 ? 2 : 1;
+  const int chans = p->Mg / *mc, taps = p->kH * p->kW;
+  const int quads = (p->outW + CONV_GROUPED_PX - 1) / CONV_GROUPED_PX;
+  int xt = quads < 32 ? quads : 32;
+  int ty_max = CONV_GROUPED_THREADS / xt;
+  int cg_max = chans;
+  for (;;) {
+    p->XT = xt;
+    p->x_tiles = (p->outW + CONV_GROUPED_PX * xt - 1) / (CONV_GROUPED_PX * xt);
+    const int tym = ty_max < p->outH ? ty_max : p->outH;
+    p->y_tiles = (p->outH + tym - 1) / tym;
+    p->TY = (p->outH + p->y_tiles - 1) / p->y_tiles;   // rows balanced over the tiles
+    int cg = CONV_GROUPED_THREADS / (xt * p->TY);
+    if (cg < 1) cg = 1;
+    if (cg > cg_max) cg = cg_max;
+    p->m_tiles = (chans + cg - 1) / cg;
+    p->CG = (chans + p->m_tiles - 1) / p->m_tiles;
+    p->PR = (p->TY - 1) * p->sH + p->kH;
+    p->PC = (CONV_GROUPED_PX * xt - 1) * p->sW + p->kW;
+    const int64_t words = static_cast<int64_t>(taps) * p->CG * *mc + static_cast<int64_t>(p->PR) * p->PC;
+    if (words * 4 <= CONV_GROUPED_SMEM) {
+      *smem_bytes = static_cast<size_t>(words) * 4;
+      break;
+    }
+    if (p->TY > 1) ty_max = (p->TY + 1) / 2;
+    else if (xt > 1) xt = (xt + 1) / 2;
+    else if (p->CG > 1) cg_max = (p->CG + 1) / 2;
+    else return 0;
+  }
+  p->tiles = g.B * G * p->m_tiles * p->y_tiles * p->x_tiles;
+  return p->XT * p->TY * p->CG;
+}
+
+template <int MC>
+__global__ void __launch_bounds__(CONV_GROUPED_THREADS)
+conv_grouped_direct_kernel(float *__restrict__ out, const float *__restrict__ in, const float *__restrict__ wts,
+                           const ConvGroupedParams p) {
+  static_assert(MC == 1 || MC == 2 || MC == 4, "channels per thread");
+  constexpr int KC = 512;   // gemm_simt_kernel.inc: 2048 / sizeof(float)
+  constexpr int PX = CONV_GROUPED_PX;
+  LB200_DYN_SMEM(float4, cg_smem4);
+  const int MB = p.CG * MC, taps = p.kH * p.kW;
+  float *ws = reinterpret_cast<float *>(cg_smem4);   // [taps][MB]
+  float *patch = ws + taps * MB;                      // [PR][PC]
+  const int nthr = p.XT * p.TY * p.CG;
+  const int tid = threadIdx.x;
+  const int cg = tid / (p.XT * p.TY), rem = tid - cg * (p.XT * p.TY);
+  const int ty = rem / p.XT, tx = rem - ty * p.XT;
+  const int patch_words = p.PR * p.PC;
+  const int64_t HW = static_cast<int64_t>(p.H) * p.W;
+  for (int64_t t = blockIdx.x; t < p.tiles; t += gridDim.x) {
+    int64_t r = t;
+    const int xt = static_cast<int>(r % p.x_tiles); r /= p.x_tiles;
+    const int yt = static_cast<int>(r % p.y_tiles); r /= p.y_tiles;
+    const int mt = static_cast<int>(r % p.m_tiles); r /= p.m_tiles;
+    const int g = static_cast<int>(r % p.G);
+    const int64_t img = r / p.G;
+    const int x0 = xt * PX * p.XT, oh0 = yt * p.TY, m0 = mt * MB;
+    const int ih0 = oh0 * p.sH - p.pH, iw0 = x0 * p.sW - p.pW;
+    const float *src = in + (img * p.C + static_cast<int64_t>(g) * p.Cg) * HW;
+    const float *wsrc = wts + (static_cast<int64_t>(g) * p.Mg + m0) * p.Cg * taps;
+    float acc[MC][PX], v[MC][PX];
+#pragma unroll
+    for (int c = 0; c < MC; ++c)
+#pragma unroll
+      for (int j = 0; j < PX; ++j) { acc[c][j] = 0.0f; v[c][j] = 0.0f; }
+    int kc = 0;   // k-steps of the current chain
+    for (int ci = 0; ci < p.Cg; ++ci) {
+      __syncthreads();   // the previous channel's patch and taps are consumed
+      for (int i = tid; i < taps * MB; i += nthr) {
+        const int tap = i / MB, mm = i - tap * MB;
+        ws[i] = m0 + mm < p.Mg ? wsrc[(static_cast<int64_t>(mm) * p.Cg + ci) * taps + tap] : 0.0f;
+      }
+      const float *sc = src + ci * HW;
+      for (int i = tid; i < patch_words; i += nthr) {
+        const int pr = i / p.PC, pc = i - pr * p.PC;
+        const int ih = ih0 + pr, iw = iw0 + pc;
+        patch[i] = (static_cast<unsigned>(ih) < static_cast<unsigned>(p.H) && static_cast<unsigned>(iw) < static_cast<unsigned>(p.W))
+                       ? sc[static_cast<int64_t>(ih) * p.W + iw] : 0.0f;
+      }
+      __syncthreads();
+      const float *prow = patch + ty * p.sH * p.PC + tx * p.sW;
+      for (int kh = 0; kh < p.kH; ++kh) {
+        for (int kw = 0; kw < p.kW; ++kw) {
+          if (kc == KC) {   // the exact kernel's next kc block: its sum is added to the previous ones
+#pragma unroll
+            for (int c = 0; c < MC; ++c)
+#pragma unroll
+              for (int j = 0; j < PX; ++j) { v[c][j] = __fadd_rn(v[c][j], acc[c][j]); acc[c][j] = 0.0f; }
+            kc = 0;
+          }
+          ++kc;
+          const float *wt = ws + (kh * p.kW + kw) * MB + cg * MC;
+          float w[MC];
+          if constexpr (MC == 4) {
+            const float4 q = *reinterpret_cast<const float4 *>(wt);
+            w[0] = q.x; w[1] = q.y; w[2] = q.z; w[3] = q.w;
+          } else if constexpr (MC == 2) {
+            const float2 q = *reinterpret_cast<const float2 *>(wt);
+            w[0] = q.x; w[1] = q.y;
+          } else {
+            w[0] = wt[0];
+          }
+          const float *px = prow + kh * p.PC + kw;
+          float x[PX];
+#pragma unroll
+          for (int j = 0; j < PX; ++j) x[j] = px[j * p.XT * p.sW];
+#pragma unroll
+          for (int c = 0; c < MC; ++c)
+#pragma unroll
+            for (int j = 0; j < PX; ++j) acc[c][j] = __fmaf_rn(w[c], x[j], acc[c][j]);
+        }
+      }
+    }
+    const int oh = oh0 + ty;
+    if (oh < p.outH) {
+#pragma unroll
+      for (int c = 0; c < MC; ++c) {
+        const int m = m0 + cg * MC + c;
+        if (m >= p.Mg) continue;
+        const int64_t co = static_cast<int64_t>(g) * p.Mg + m;
+        float *orow = out + ((img * p.G * p.Mg + co) * p.outH + oh) * p.outW;
+#pragma unroll
+        for (int j = 0; j < PX; ++j) {
+          const int ow = x0 + tx + j * p.XT;
+          if (ow >= p.outW) continue;
+          float y = __fadd_rn(v[c][j], acc[c][j]);
+          if (p.bias != nullptr || p.act != 0) y = simt_bias_act(y, p.bias, 1, p.act, co, 0);
+          orow[ow] = y;
+        }
+      }
+    }
+  }
+}
 
 }  // namespace lb200

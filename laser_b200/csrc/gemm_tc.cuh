@@ -220,8 +220,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
         if constexpr (BATCHED) {
           const int bz = t / tiles_pp;
           t -= bz * tiles_pp;
-          za = bz * p.map_b_a;
-          zb = bz * p.map_b_b;
+          za = bz % p.period_a;
+          zb = bz % p.period_b;
         }
         tile_coords(t, p.num_m_blocks, p.num_n_blocks, p.raster_g, mb, nb);
         const int m0 = mb * TC_BLOCK_M;
@@ -267,9 +267,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
       if (u < 0) break;
       int t, sp, mb, nb, kb_lo, kb_hi;
       decode_unit(u, t, sp, kb_lo, kb_hi);
-      int bz = 0;   // problem of the tile
+      int bz = 0, za = 0, zb = 0;   // problem of the tile, its slices of A (scale words, per-row bias) and B (scale words)
       if constexpr (BATCHED) {
         bz = t / tiles_pp;
+        za = bz % p.period_a;
+        zb = bz % p.period_b;
         int tl = t - bz * tiles_pp;
         tile_coords(tl, p.num_m_blocks, p.num_n_blocks, p.raster_g, mb, nb);
       } else {
@@ -286,11 +288,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
       if constexpr (SCALED) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-          if (row0 + 8 * h < p.M) amax_row[h] = p.amax_a[(BATCHED ? bz * p.amax_bs_a : 0) + row0 + 8 * h];
+          if (row0 + 8 * h < p.M) amax_row[h] = p.amax_a[(BATCHED ? za * p.amax_bs_a : 0) + row0 + 8 * h];
 #pragma unroll
         for (int j = 0; j < 2 * TC_BLOCK_N / 8; ++j) {
           const int64_t c = col0 + 8 * (j >> 1) + (j & 1);
-          amax_col[j] = c < p.N ? p.amax_b[(BATCHED ? bz * p.amax_bs_b : 0) + c] : 0u;
+          amax_col[j] = c < p.N ? p.amax_b[(BATCHED ? zb * p.amax_bs_b : 0) + c] : 0u;
         }
       }
       float run[TC_ACC_REGS];  // running sums of this thread's fragment (registers)
@@ -355,7 +357,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
       for (int h = 0; h < 2; ++h) {
         const int64_t row = row0 + 8 * h;
         if (!split_unit && row >= p.M) continue;
-        const float row_bias = (has_epi && p.epi.bias && p.epi.bias_per_row) ? p.epi.bias[row] : 0.0f;
+        const float row_bias =
+            (has_epi && p.epi.bias && p.epi.bias_per_row) ? p.epi.bias[(BATCHED ? za * p.bias_bs : 0) + row] : 0.0f;
         OutT *crow = split_unit ? nullptr : reinterpret_cast<OutT *>(p.C) + (BATCHED ? bz * p.bsC : 0) + row * p.rsC;
 #pragma unroll
         for (int i = 0; i < TC_BLOCK_N / 8; ++i) {

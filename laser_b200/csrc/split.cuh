@@ -1093,12 +1093,14 @@ pack_general_kernel(const T *__restrict__ src, int64_t R, int64_t Cc, int64_t sr
 // Second half of a split-K GEMM (tc_params.h): C <- act(alpha * sum_s ws[s][i] + beta * C + bias) over the split tiles
 // n_direct + i, i < n_tail, planes added in the fixed order s = 0 .. S-1 (deterministic).  ws: [S][n_tail][TC_BLOCK_M][TC_BLOCK_N]
 // fp32, tile-local.  Item = four consecutive columns of one tile row.  BATCHED: tile t of the launch is tile t % (num_m * num_n)
-// of problem t / (num_m * num_n), whose C starts bsC elements after the previous problem's (tc_params.h).
+// of problem t / (num_m * num_n), whose C starts bsC elements after the previous problem's and whose bias starts
+// (problem % period_a) * bias_bs elements into `bias` (tc_params.h).
 template <bool BATCHED = false>
 __global__ void __launch_bounds__(256)
 splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n_direct, int num_m, int num_n, int raster_g,
                           int64_t M, int64_t N, float alpha, float beta, float *__restrict__ C, int64_t rsC,
-                          int64_t csC, const float *__restrict__ bias, int bias_per_row, int act, int64_t bsC = 0) {
+                          int64_t csC, const float *__restrict__ bias, int bias_per_row, int act, int64_t bsC = 0, int period_a = 1,
+                          int64_t bias_bs = 0) {
   constexpr int V = TC_BLOCK_N / 4;   // float4 per tile row
   const int64_t per_tile = static_cast<int64_t>(TC_BLOCK_M) * V;
   const int64_t total = static_cast<int64_t>(n_tail) * per_tile;
@@ -1110,10 +1112,12 @@ splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n
     const int r_l = static_cast<int>(rem / V), c4 = static_cast<int>(rem - static_cast<int64_t>(r_l) * V);
     int mb, nb, t = n_direct + ti;
     float *Cb = C;
+    const float *bb = bias;
     if constexpr (BATCHED) {
       const int b = t / (num_m * num_n);
       t -= b * (num_m * num_n);
       Cb += b * bsC;
+      if (bb) bb += (b % period_a) * bias_bs;
     }
     tile_coords(t, num_m, num_n, raster_g, mb, nb);
     const int64_t r = static_cast<int64_t>(mb) * TC_BLOCK_M + r_l, c = static_cast<int64_t>(nb) * TC_BLOCK_N + 4 * c4;
@@ -1131,8 +1135,8 @@ splitk_tail_reduce_kernel(const float *__restrict__ ws, int S, int n_tail, int n
       if (c + e < N) {
         float v = alpha * sv[e];
         if (beta != 0.0f) v = fmaf(beta, dst[e * csC], v);
-        if (bias != nullptr || act != 0) {
-          if (bias) v += bias_per_row ? bias[r] : bias[c + e];
+        if (bb != nullptr || act != 0) {
+          if (bb) v += bias_per_row ? bb[r] : bb[c + e];
           if (act == 1) v = fmaxf(v, 0.0f);
           else if (act == 2) v = tanhf(v);
           else if (act == 3) v = 1.0f / (1.0f + expf(-v));

@@ -70,12 +70,15 @@ struct TcParams {
   unsigned int *sched = nullptr;
   // batched launch (gemm_tc_kernel<..., BATCHED = true>): `batch` problems of M x N x K.  Tile t of the launch is tile
   // t % (num_m_blocks * num_n_blocks) of problem t / (num_m_blocks * num_n_blocks); split-K and the raster order apply to
-  // these tiles as above.  Problem b reads slice b * map_b_a (b * map_b_b) of A's (B's) rank-3 tensor maps -- 0 for an
-  // operand the batch shares --, writes C + b * bsC and reads its scale words b * amax_bs_a (b * amax_bs_b) further on.
+  // these tiles as above.  An operand repeats with a period: problem b reads slice b % period_a (b % period_b) of A's (B's)
+  // rank-3 tensor maps and its scale words (b % period_a) * amax_bs_a ((b % period_b) * amax_bs_b) further on -- period 1 for
+  // an operand the batch shares, `batch` for one each problem owns, G for the filters of a G-group convolution --, and writes
+  // C + b * bsC.  A per-row bias follows A: problem b reads it (b % period_a) * bias_bs further on (0: shared by the batch).
   int batch = 1;
-  int map_b_a = 0, map_b_b = 0;
+  int period_a = 1, period_b = 1;
   int64_t bsC = 0;
   int64_t amax_bs_a = 0, amax_bs_b = 0;
+  int64_t bias_bs = 0;
 };
 
 // raster order of the output tiles: groups of G m-blocks sweep n together, so that the concurrently resident tiles (132 of

@@ -9,6 +9,8 @@
     im2col, conv2d_im2col                         conv2d_im2col.nim:44-166
     conv2d_fused                                  conv2d_im2col.nim:95-166 + bias + activation, im2col folded into the
                                                   GEMM's operand preparation (README.md:251)
+    conv2d_grouped_fused                          conv2d_fused with groups > 1 (torch.nn.Conv2d(groups=G)): depthwise and
+                                                  grouped layers in one call
     conv2d_filter_grad_fused                      its filter gradient, derivative op on grad_output and the window gather
                                                   folded into the operand preparation (README.md:244-245, :251)
     conv2d_nhwc_filter_grad_fused                 the filter gradient of conv2d_nhwc_fused: NHWC images and gradients, the
@@ -34,7 +36,7 @@ from .tensor import _ITEMSIZE, Tensor
 FOREACH_OPS = {"copy": 0, "fill": 1, "scale": 2, "add": 3, "sub": 4, "mul": 5, "fma": 6, "axpy": 7, "bench": 8}
 
 __all__ = ["forEach", "FOREACH_OPS", "transpose2D_copy", "transpose2D_batched", "nchw2nhwc", "nhwc2nchw", "conv2d_out_shape",
-           "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "conv2d_filter_grad_fused", "conv2d_input_grad_fused",
+           "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "conv2d_grouped_fused", "conv2d_filter_grad_fused", "conv2d_input_grad_fused",
            "gemm_strided_batched", "copyFrom"]
 
 _i64 = ctypes.c_int64
@@ -153,6 +155,24 @@ def conv2d_fused(output, input, ishape, kernel, kshape, padding, strides, bias=N
     stream = _current_stream() if stream is None else stream
     check(lib().laser_b200_conv2d_f32_fused_dev(po, pi, _i4(ishape), pk, _i4(kshape), _i2(padding), _i2(strides),
                                                 ctypes.byref(epi), int(path), stream))
+
+
+def conv2d_grouped_fused(output, input, ishape, kernel, kshape, padding, strides, groups, bias=None, activation="none",
+                         path=PATH_AUTO, stream=None):
+    """conv2d_fused with `groups` groups, as torch.nn.functional.conv2d(groups=groups), on float32 DEVICE buffers: NCHW in and
+    out, kernel [c_out, c_in / groups, kH, kW] (kshape in that order).  Output channel co of group g = co // (c_out / groups)
+    sees input channels g * c_in / groups .. (g + 1) * c_in / groups - 1.  bias: one per output channel.  activation: none |
+    relu | tanh | sigmoid.  One call for every group: a direct CUDA-core kernel on the exact path (depthwise and narrow
+    groups), one batched tensor-core GEMM launch on the others.  groups=1 is conv2d_fused."""
+    po, pi, pk = _dev_f32(output), _dev_f32(input), _dev_f32(kernel)
+    epi = Epilogue()
+    if bias is not None:
+        epi.bias = _dev_f32(bias)
+    epi.bias_per_row = 1
+    epi.activation = {"none": 0, "relu": 1, "tanh": 2, "sigmoid": 3}[activation]
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_grouped_f32_fused_dev(po, pi, _i4(ishape), pk, _i4(kshape), _i2(padding), _i2(strides), int(groups),
+                                                        ctypes.byref(epi), int(path), stream))
 
 
 def conv2d_nhwc_fused(output, input, ishape, kernel, kshape, padding, strides, bias=None, activation="none", path=PATH_AUTO,

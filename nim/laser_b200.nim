@@ -288,6 +288,10 @@ proc laser_b200_conv2d_im2col_f32*(output, input: ptr float32, ishape: ptr array
 proc laser_b200_conv2d_f32_fused_dev*(output, input: ptr float32, ishape: ptr array[4, int64], kernel: ptr float32,
                                       kshape: ptr array[4, int64], padding, strides: ptr array[2, int64],
                                       epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
+# the same with groups > 1 (torch.nn.Conv2d(groups=...)): kernel [c_out][c_in / groups][kH][kW]; groups = 1 is the call above
+proc laser_b200_conv2d_grouped_f32_fused_dev*(output, input: ptr float32, ishape: ptr array[4, int64], kernel: ptr float32,
+                                              kshape: ptr array[4, int64], padding, strides: ptr array[2, int64], groups: int64,
+                                              epi: ptr LaserB200Epilogue, path: cint, stream: pointer): cint
 # the same in channels-last layout (conv2d_mec.nim): NHWC input and output, the filter matrix [kH*kW*c_in][c_out] read with
 # kernelStrides ({c_out, 1} for kernel_to_hwcc's layout); one GEMM over the windows prepared from the images
 proc laser_b200_conv2d_nhwc_f32_fused_dev*(output, input: ptr float32, ishape: ptr array[4, int64], kernel: ptr float32,
