@@ -582,6 +582,41 @@ int laser_b200_conv2d_input_grad_f32_fused_dev(float *grad_input, const int64_t 
                                                const float *kernel, const int64_t kshape[4], const int64_t padding[2],
                                                const int64_t strides[2], float alpha, float beta,
                                                const laser_b200_operand_op *op, int path, void *stream);
+/* Input gradient of the grouped fused convolution (torch.nn.grad.conv2d_input(groups=G)): for every image n and group g, with
+ * Cg = c_in / groups, Mg = c_out / groups, T = kH * kW and K' = Mg * T,
+ *   grad_input_n[g * Cg + ci] <- alpha * sum_{co < Mg, t < T} W'_g[ci][co * T + t] * B_{n,g}[pixel][co * T + t]
+ *                                + beta * grad_input_n[g * Cg + ci],
+ *   W'_g[ci][co * T + t] = kernel[g * Mg + co][ci][T - 1 - t]   (rotated by 180 degrees, channel axes swapped, per group)
+ * where B_{n,g} is conv2d_input_grad_f32_fused_dev's transposed window over op(grad_output_n) restricted to channels g * Mg ..
+ * (g + 1) * Mg - 1: zero-dilated by the strides, padded by kH - 1 - pH, a hole 0 (never op(0)).  The shapes and argument rules
+ * are conv2d_grouped_f32_fused_dev's: grad_input dense NCHW of shape ishape, grad_output dense NCHW [n][c_out][outH][outW],
+ * kernel torch's grouped weight [c_out][c_in / groups][kH][kW].  op (NULL: none) as for conv2d_input_grad_f32_fused_dev, a
+ * derivative op's aux dense NCHW like grad_output (auxRowStride = outH * outW, auxColStride = 1).  No bias gradient.
+ *   groups == 1 is laser_b200_conv2d_input_grad_f32_fused_dev: the same bits, launches and last_path on every path.
+ *   PATH_SIMT (exact): the direct kernel of the grouped forward call run over the transposed geometry, ONE launch for every
+ *   image and group, the filters read rotated in place, no copy and no workspace.  Each output is the exact GEMM's fmaf chain
+ *   (restarted every 512 k-steps) with its alpha / beta epilogue, holes and padding multiplied as zeros (an Inf filter tap gives
+ *   NaN wherever the GEMM over the windows does), so grad_input is bit for bit G calls of conv2d_input_grad_f32_fused_dev on
+ *   PATH_SIMT over contiguous per-group copies -- the oracle's gemm_strided(W'_g, rows_{n,g}, alpha, beta) per image and group.
+ *   Tensor-core paths: W' of every group written once per call into library workspace (one launch), then the n * G problems
+ *   -- image n's dY channel slice of group g, its dX channel slice -- are ONE batched GEMM per chunk of whole images
+ *   (LASER_B200_BATCH_WS_MB) whose A repeats every G problems: one filter copy, then 3 launches per chunk (filter rows, window
+ *   rows, GEMM; split-K adds a reduce), whatever n and G.  1 x 1 kernels with unit strides and no padding read grad_output in
+ *   place and the filters transposed, no copy.  The bits equal G calls of conv2d_input_grad_f32_fused_dev on contiguous
+ *   per-group copies on the same path whenever neither side is split along K: with the default LASER_B200_KC a split needs 8
+ *   accumulation blocks (K' >= 897 on f16x3 and tf32x3; tf32x1 never splits), so K' <= 896 suffices.  Beyond that the result
+ *   is within the per-element bound of the tensor-core products.
+ *   PATH_AUTO: conv2d_input_grad_f32_fused_dev's decision for the per-group geometry (n * G images, M = Cg, K' = Mg * T): the
+ *   exact path when Cg < 64 or K' < 64 (every depthwise layer), else the tensor-core path of one group.
+ *   n = 0: LASER_B200_OK, nothing launched, grad_input untouched.
+ *   LASER_B200_EINVAL, before anything is launched: groups < 1; c_in or c_out not a multiple of groups; kshape[1] * groups !=
+ *   c_in; geometry errors; an unknown path or op; a derivative op without aux or with other aux strides; a NULL pointer.
+ *   LASER_B200_EUNSUPPORTED: K' beyond int32; on a tensor-core path, n * G problems (one chunk's at least) or their tiles
+ *   beyond int32; on the exact path, a kernel window too large for the direct kernel's shared-memory tile. */
+int laser_b200_conv2d_grouped_input_grad_f32_fused_dev(float *grad_input, const int64_t ishape[4], const float *grad_output,
+                                                       const float *kernel, const int64_t kshape[4], const int64_t padding[2],
+                                                       const int64_t strides[2], int64_t groups, float alpha, float beta,
+                                                       const laser_b200_operand_op *op, int path, void *stream);
 /* Input gradient of the channels-last fused convolution (conv2d_nhwc_f32_fused_dev's layouts; the reference has no backward
  * convolution):
  *   grad_input[j][ci] <- alpha * sum_k' R[j][k'] * W'^T[ci][k'] + beta * grad_input[j][ci],  j = n * H * W + ih * W + iw

@@ -18,6 +18,7 @@
 //   conv2d_im2col                                     benchmarks/convolution/conv2d_common.nim:6-45,
 //                                                     conv2d_im2col.nim:8-166
 //   laser::conv2d_grouped_fused_dev                   torch.nn.Conv2d(groups=G) on device buffers
+//   laser::conv2d_grouped_input_grad_dev              torch.nn.grad.conv2d_input(groups=G) on device buffers
 #pragma once
 
 #include <cstdint>
@@ -254,6 +255,17 @@ inline void conv2d_grouped_fused_dev(float *output, const float *input, TensorSh
   const int64_t is[4] = {ishape.n, ishape.c, ishape.h, ishape.w}, ks[4] = {kshape.c_out, kshape.c_in, kshape.kH, kshape.kW};
   const int64_t pd[2] = {padding.h, padding.w}, st[2] = {strides.h, strides.w};
   check(laser_b200_conv2d_grouped_f32_fused_dev(output, input, is, kernel, ks, pd, st, groups, epi, path, stream));
+}
+// its input gradient (laser_b200_conv2d_grouped_input_grad_f32_fused_dev): grad_input <- alpha * conv_transpose(op(grad_output),
+// kernel) + beta * grad_input per group; op NULL = none; stream NULL = the library's stream, synchronous
+inline void conv2d_grouped_input_grad_dev(float *grad_input, TensorShape ishape, const float *grad_output, const float *kernel,
+                                          KernelShape kshape, Padding padding, Strides strides, int64_t groups, float alpha = 1.0f,
+                                          float beta = 0.0f, const laser_b200_operand_op *op = nullptr,
+                                          int path = LASER_B200_PATH_AUTO, void *stream = nullptr) {
+  const int64_t is[4] = {ishape.n, ishape.c, ishape.h, ishape.w}, ks[4] = {kshape.c_out, kshape.c_in, kshape.kH, kshape.kW};
+  const int64_t pd[2] = {padding.h, padding.w}, st[2] = {strides.h, strides.w};
+  check(laser_b200_conv2d_grouped_input_grad_f32_fused_dev(grad_input, is, grad_output, kernel, ks, pd, st, groups, alpha, beta, op,
+                                                           path, stream));
 }
 
 }  // namespace laser

@@ -10,7 +10,7 @@ from .gemm import (DevPtr, fill_uniform_f32, gemm_strided, gemm_strided_batch_re
                    gemm_strided_fused, get_f32_mode, init, last_path,
                    launch_count, profile_begin, profile_end, set_f32_mode, shutdown,
                    synchronize)
-from .layers import (FOREACH_OPS, conv2d_filter_grad_fused, conv2d_fused, conv2d_grouped_fused, conv2d_im2col, conv2d_input_grad_fused, conv2d_nhwc_fused,
+from .layers import (FOREACH_OPS, conv2d_filter_grad_fused, conv2d_fused, conv2d_grouped_fused, conv2d_grouped_input_grad_fused, conv2d_im2col, conv2d_input_grad_fused, conv2d_nhwc_fused,
                      conv2d_nhwc_filter_grad_fused, conv2d_nhwc_input_grad_fused, conv2d_out_shape, copyFrom, forEach, gemm_strided_batched, im2col, im2col_workspace_size, nchw2nhwc, nhwc2nchw, transpose2D_batched,
                      transpose2D_copy)
 from .prepacked import (alloc_packed, gemm_packed, gemm_packedB, gemm_prepackA, gemm_prepackA_mem_required,

@@ -138,6 +138,8 @@ SIGNATURES = {
                                                                         f32, ctypes.POINTER(OperandOp), ctypes.c_int, vp]),
     "laser_b200_conv2d_input_grad_f32_fused_dev": (ctypes.c_int, [vp, i64 * 4, vp, vp, i64 * 4, i64 * 2, i64 * 2, f32, f32,
                                                                   ctypes.POINTER(OperandOp), ctypes.c_int, vp]),
+    "laser_b200_conv2d_grouped_input_grad_f32_fused_dev": (ctypes.c_int, [vp, i64 * 4, vp, vp, i64 * 4, i64 * 2, i64 * 2, i64, f32,
+                                                                          f32, ctypes.POINTER(OperandOp), ctypes.c_int, vp]),
     "laser_b200_conv2d_nhwc_input_grad_f32_fused_dev": (ctypes.c_int, [vp, i64 * 4, vp, vp, i64 * 4, i64 * 2, i64 * 2, i64 * 2, f32,
                                                                        f32, ctypes.POINTER(OperandOp), ctypes.c_int, vp]),
     "laser_b200_copy_views": (ctypes.c_int, [ctypes.POINTER(TensorView), ctypes.POINTER(TensorView), vp]),

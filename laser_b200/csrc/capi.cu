@@ -128,8 +128,8 @@ struct Ctx {
   Buffer splitk;     // split-K partial-sum planes
   Buffer bpanels;    // row-sharded products: B prepared, panel-major (capi_multi.inc: rowshard_prepared)
   Buffer layer_ws;   // im2col workspace of the host-pointer convolution
-  Buffer tfilt;      // the input gradients' rotated filters, under tfilt_mu for a whole call: W' (conv2d_input_grad_dev) or W'^T
-                     // (conv2d_nhwc_input_grad_dev)
+  Buffer tfilt;      // the input gradients' rotated filters, under tfilt_mu for a whole call: W' (conv2d_input_grad_dev), W'^T
+                     // (conv2d_nhwc_input_grad_dev) or W'_g of every group (conv2d_grouped_input_grad_dev, tensor-core paths)
   Buffer f16s;       // F16X3 mode: fp32 bits of max_k |a| per row of A (words [0, M)) and of max_k |b| per column of B (from
                      // f16_b_off on), written and read on the device
   Buffer sched;      // kSchedSlots x {next unit, CTAs done}: the kernel re-zeroes its slot when it ends
@@ -137,7 +137,7 @@ struct Ctx {
   cudaEvent_t ws_free = nullptr;  // recorded after the last kernel that reads ws[]
   std::mutex mu;       // workspace + tensor-map construction
   std::mutex host_mu;  // staging buffers of the host-pointer entry points
-  std::mutex tfilt_mu; // tfilt: written once per call of either input gradient, read by every chunk's product (each takes mu
+  std::mutex tfilt_mu; // tfilt: written once per call of an input gradient, read by every chunk's product (each takes mu
                        // itself)
   std::atomic<bool> ready{false};
 };
@@ -1540,6 +1540,18 @@ int launch_copy(Ctx &c, void *dst, const void *src, const CopyParams &p, cudaStr
 // ---------------------------------------------------------------------------------------
 //   convolution input gradient: the forward product over the output gradients as a transposed, dilated im2col source
 // ---------------------------------------------------------------------------------------
+// The transposed geometry of the input gradients: the output gradients (Cout channels of outH x outW) as the source, zero-dilated
+// by the forward strides and padded by kH - 1 - pH, stride 1, windows at the input's H x W pixels and C output channels
+ConvGeom transposed_geom(const ConvGeom &g) {
+  ConvGeom gt = g;
+  gt.C = g.Cout; gt.H = g.outH; gt.W = g.outW; gt.Cout = g.C;
+  gt.pH = g.kH - 1 - g.pH; gt.pW = g.kW - 1 - g.pW;
+  gt.sH = gt.sW = 1;
+  gt.dH = g.sH; gt.dW = g.sW;
+  gt.outH = g.H; gt.outW = g.W;
+  return gt;
+}
+
 // laser_b200_conv2d_input_grad_f32_fused_dev (capi_layers.inc checks the geometry):
 //   grad_input_n <- alpha * W' * B_n + beta * grad_input_n,  W'[ci][(co, kh', kw')] = W[co][ci][kH-1-kh'][kW-1-kw']
 // B_n: grad_output_n (op applied) as the im2col source of the transposed geometry gt -- C = Cout, H x W = outH x outW,
@@ -1560,12 +1572,7 @@ int conv2d_input_grad_dev(float *grad_input, const ConvGeom &g, const float *gra
   if (g.B == 0) return LASER_B200_OK;
   if (!grad_input || !grad_output || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
   if (g.Cout > INT32_MAX / khw) return set_error(LASER_B200_EUNSUPPORTED, "c_out * kH * kW beyond 2^31");
-  ConvGeom gt = g;
-  gt.C = g.Cout; gt.H = g.outH; gt.W = g.outW; gt.Cout = g.C;
-  gt.pH = g.kH - 1 - g.pH; gt.pW = g.kW - 1 - g.pW;
-  gt.sH = gt.sW = 1;
-  gt.dH = g.sH; gt.dW = g.sW;
-  gt.outH = g.H; gt.outW = g.W;
+  ConvGeom gt = transposed_geom(g);
   const int64_t K = gt.K();
   // dX_n = W^T * dY_n for a 1 x 1 kernel with unit strides and no padding: W read transposed, no copy
   if (khw == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0)
@@ -1586,6 +1593,91 @@ int conv2d_input_grad_dev(float *grad_input, const ConvGeom &g, const float *gra
   float *wt = static_cast<float *>(c->tfilt.ptr);
   if ((rc = launch_copy<uint32_t>(*c, wt, kernel + khw - 1, cp, s))) return rc;
   return conv_windows_dev(gt, alpha, wt, lda, 1, grad_output, beta, grad_input, opB, Epilogue(), path, stream);
+}
+
+// laser_b200_conv2d_grouped_input_grad_f32_fused_dev (capi_layers.inc checks the geometry and the groups; groups == 1 never
+// comes here): conv2d_input_grad_dev per group, G groups of Cg = C / G input and Mg = Cout / G output channels, T = kH * kW,
+// K' = Mg * T.  gt is the transposed geometry of the whole layer (Cout source channels, C output channels), gtp that of one
+// group -- n * G images of Mg channels, Cout = Cg --: problem b = i * G + g reads image i's dY channel slice of group g (one
+// image of gtp, the NCHW slices are Mg * outH * outW apart; the aux likewise), writes dX channels g * Cg .. (one output image
+// of gtp) and reads the rotated filters W'_g of group b % G.
+//   PATH_AUTO: conv_auto_path over gtp.  The exact path is the direct kernel over gt (gemm_simt.cuh: conv_grouped_direct_kernel
+//   with GRAD), one launch, the filters read rotated in place.  The tensor-core paths are the batched fused product over gtp
+//   with A = W' copied once per call into tfilt as G problems of [Cg][round_up(K', 4)], periodic with period G
+//   (batched_fused_dev), and B the dilated, op'd windows of dY (split.cuh: Im2colGradSrc); a 1 x 1 kernel with unit strides
+//   and no padding reads dY in place and the filters transposed, no copy.
+int conv2d_grouped_input_grad_dev(float *grad_input, const ConvGeom &g, int64_t groups, const float *grad_output, const float *kernel,
+                                  float alpha, float beta, const laser_b200_operand_op *op_in, int path, void *stream) {
+  int rc;
+  if ((rc = check_f32_path(path))) return rc;
+  OperandOp op;
+  const OperandOp *opB;
+  if ((rc = operand_op_of(op_in, true, &op, &opB))) return rc;
+  const int64_t P = g.outHW(), khw = g.kH * g.kW;
+  if (opB && opB->aux && (opB->aux_sr != 1 || opB->aux_sc != P))
+    return set_error(LASER_B200_EINVAL, "the aux tensor of op %d must be dense like grad_output: strides (%lld, 1), not (%lld, %lld)",
+                     opB->op, (long long)P, (long long)opB->aux_sc, (long long)opB->aux_sr);
+  if (g.B == 0) return LASER_B200_OK;
+  if (!grad_input || !grad_output || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
+  const int64_t Cg = g.C / groups, Mg = g.Cout / groups;
+  if (Mg > INT32_MAX / khw) return set_error(LASER_B200_EUNSUPPORTED, "c_out / groups * kH * kW beyond 2^31");
+  ConvGeom gt = transposed_geom(g);
+  ConvGeom gtp = gt;
+  gtp.B = g.B * groups;
+  gtp.C = Mg;
+  gtp.Cout = Cg;
+  if (path == LASER_B200_PATH_AUTO) path = conv_auto_path(gtp, Epilogue());
+  Ctx *c;
+  if ((rc = get_ctx(&c))) return rc;
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  if (path == LASER_B200_PATH_SIMT) {
+    ConvGroupedGradParams p;
+    int mc;
+    size_t smem;
+    const int threads = conv_grouped_plan(gt, groups, nullptr, 0, &p, &mc, &smem);
+    if (threads == 0)
+      return set_error(LASER_B200_EUNSUPPORTED, "grouped convolution input gradient: a %lld x %lld kernel window does not fit in "
+                       "shared memory", (long long)g.kH, (long long)g.kW);
+    p.dH = static_cast<int>(g.sH);
+    p.dW = static_cast<int>(g.sW);
+    p.alpha = alpha;
+    p.beta = beta;
+    p.op = opB ? opB->op : 0;
+    p.aux = opB ? opB->aux : nullptr;
+    const int grid = grid_for(*c, p.tiles, 2048 / threads);
+    if (mc == 4) conv_grouped_direct_kernel<4, true><<<grid, threads, smem, s>>>(grad_input, grad_output, kernel, p);
+    else if (mc == 2) conv_grouped_direct_kernel<2, true><<<grid, threads, smem, s>>>(grad_input, grad_output, kernel, p);
+    else conv_grouped_direct_kernel<1, true><<<grid, threads, smem, s>>>(grad_input, grad_output, kernel, p);
+    COUNT_LAUNCH();
+    CHECK_LAUNCH();
+  } else {
+    const int64_t M = Cg, N = gtp.outHW(), K = gtp.K(), image = Mg * g.outH * g.outW;
+    if (khw == 1 && g.sH == 1 && g.sW == 1 && g.pH == 0 && g.pW == 0) {
+      // dX_{n,g} = W_g^T * dY_{n,g}: group g's filters [Mg][Cg] read transposed, dY in place
+      const laser_b200_batch_strides bs{Mg * Cg, image, M * N, 0, image};
+      if ((rc = batched_fused_dev(gtp.B, M, N, K, alpha, kernel, 1, Cg, grad_output, N, 1, beta, grad_input, N, 1, &bs, nullptr, opB,
+                                  Epilogue(), path, s, nullptr, groups)))
+        return rc;
+    } else {
+      // W' of every group once per call into tfilt (held for the whole call), K-major rows 16 bytes apart, read in place by
+      // every chunk's product; the copy waits for the last kernel that read the buffer (ws_free)
+      std::lock_guard<std::mutex> lk(c->tfilt_mu);
+      const int64_t lda = round_up(K, 4);
+      if ((rc = ensure(c->tfilt, static_cast<size_t>(g.C * lda) * sizeof(float)))) return rc;
+      CUDA_TRY(cudaStreamWaitEvent(s, c->ws_free, 0));
+      const int64_t shape[4] = {groups, Cg, Mg, khw}, dst_st[4] = {Cg * lda, lda, khw, 1}, src_st[4] = {Mg * Cg * khw, khw, Cg * khw, -1};
+      CopyParams cp;
+      copy_plan(4, shape, dst_st, src_st, &cp);
+      float *wt = static_cast<float *>(c->tfilt.ptr);
+      if ((rc = launch_copy<uint32_t>(*c, wt, kernel + khw - 1, cp, s))) return rc;
+      const laser_b200_batch_strides bs{Cg * lda, image, M * N, 0, image};
+      if ((rc = batched_fused_dev(gtp.B, M, N, K, alpha, wt, lda, 1, grad_output, N, 1, beta, grad_input, N, 1, &bs, nullptr, opB,
+                                  Epilogue(), path, s, &gtp, groups)))
+        return rc;
+    }
+  }
+  g_last_path = path;
+  return finish(*c, static_cast<cudaStream_t>(stream), s);
 }
 
 // laser_b200_conv2d_nhwc_input_grad_f32_fused_dev (capi_layers.inc checks the geometry): NHWC output gradients and input
@@ -1614,12 +1706,7 @@ int conv2d_nhwc_input_grad_dev(float *grad_input, const ConvGeom &g, const float
   if (g.B == 0) return LASER_B200_OK;
   if (!grad_input || !grad_output || !kernel) return set_error(LASER_B200_EINVAL, "null pointer");
   if (g.Cout > INT32_MAX / khw) return set_error(LASER_B200_EUNSUPPORTED, "c_out * kH * kW beyond 2^31");
-  ConvGeom gt = g;
-  gt.C = g.Cout; gt.H = g.outH; gt.W = g.outW; gt.Cout = g.C;
-  gt.pH = g.kH - 1 - g.pH; gt.pW = g.kW - 1 - g.pW;
-  gt.sH = gt.sW = 1;
-  gt.dH = g.sH; gt.dW = g.sW;
-  gt.outH = g.H; gt.outW = g.W;
+  ConvGeom gt = transposed_geom(g);
   gt.nhwc = true;
   if (path == LASER_B200_PATH_AUTO) path = conv_auto_path(gt, Epilogue());
   if (is_tc_mode(path) && gt.outHW() > 0x7fffffffLL / g.B)
@@ -2257,6 +2344,7 @@ int laser_b200_fill_uniform_f32_dev(float *dst_dev, int64_t n, uint64_t seed, fl
 #define LB200_CONV2D_FILTER_GRAD_F32 conv2d_filter_grad_dev
 #define LB200_CONV2D_NHWC_FILTER_GRAD_F32 conv2d_nhwc_filter_grad_dev
 #define LB200_CONV2D_INPUT_GRAD_F32 conv2d_input_grad_dev
+#define LB200_CONV2D_GROUPED_INPUT_GRAD_F32 conv2d_grouped_input_grad_dev
 #define LB200_CONV2D_NHWC_INPUT_GRAD_F32 conv2d_nhwc_input_grad_dev
 #include "capi_layers.inc"
 #include "capi_multi.inc"

@@ -25,6 +25,7 @@
 
 #include "layers.cuh"
 #include "ptx.cuh"
+#include "split.cuh"
 
 namespace lb200 {
 
@@ -518,6 +519,19 @@ template <int MT> constexpr size_t ska_smem_bytes() { return (static_cast<size_t
 // each input channel ci of the group the CTA stages in shared memory the zero-padded input rows and columns the tile
 // reads, [PR][PC], and the tile's filter taps of ci, [kH * kW][CG * MC] (a thread's MC weights of one tap in one 4-, 8- or
 // 16-byte load); the FMAs then read only shared memory.  Depthwise layers (Cg = 1) stage one channel per CTA tile.
+//
+// GRAD = true: the exact path of laser_b200_conv2d_grouped_input_grad_f32_fused_dev, the same tiles and chains over the
+// transposed geometry of the input gradient (capi.cu: conv2d_grouped_input_grad_dev).  `in` is dY, its C = c_out channels
+// (Cg = c_out / G per group) zero-dilated by (dH, dW) = the forward strides and padded by kH - 1 - pH (negative: cropped),
+// stride 1; `out` is dX, Mg = c_in / G channels per group.  The three differences, each under `if constexpr`:
+//   - patch word (h, w) of the dilated plane is op(dY[h / dH][w / dW]) (split.cuh: operand_op, the aux read at dY's offset)
+//     when h >= 0, h % dH == 0 and h / dH < H (columns likewise), else 0: a hole is 0, never op(0), and its taps are
+//     fmaf(w, 0, acc) as the padding's are;
+//   - the taps of source channel co for output channel m are the caller's filters rotated and transposed in place,
+//     wts[(g * Cg + co) * Mg * T + m * T + T - 1 - t], T = kH * kW: the rows W'_g of the input gradient, no copy;
+//   - the exact kernel's alpha / beta epilogue per KC block (beta1 in gemm_simt_kernel.inc): v starts at 0 (beta = 0: dX
+//     not read), dX or dX * beta, and every block adds acc or alpha * acc; no bias, no activation.
+// So dX is bit for bit the oracle's gemm_strided(W'_g, rows_{n,g}, alpha, beta) per image and group.
 // ---------------------------------------------------------------------------
 constexpr int CONV_GROUPED_PX = 4;                 // output pixels per thread, XT apart along a row
 constexpr int CONV_GROUPED_THREADS = 256;          // most threads of a CTA
@@ -532,6 +546,14 @@ struct ConvGroupedParams {
   int64_t tiles;                     // images * G * m_tiles * y_tiles * x_tiles
   const float *bias;
   int act;
+};
+// the input gradient's (GRAD) parameters: the plan's, and what the caller sets after it -- the source's dilation, the scalars
+// and the op on the source (aux laid out like it, NULL: none)
+struct ConvGroupedGradParams : ConvGroupedParams {
+  int dH, dW;
+  float alpha, beta;
+  int op;
+  const float *aux;
 };
 
 // Host side: the tile of a geometry (C, Cout, ... of the whole layer; G groups).  *mc = channels per thread (1, 2 or 4:
@@ -580,10 +602,10 @@ inline int conv_grouped_plan(const ConvGeom &g, int64_t G, const float *bias, in
   return p->XT * p->TY * p->CG;
 }
 
-template <int MC>
+template <int MC, bool GRAD = false>
 __global__ void __launch_bounds__(CONV_GROUPED_THREADS)
 conv_grouped_direct_kernel(float *__restrict__ out, const float *__restrict__ in, const float *__restrict__ wts,
-                           const ConvGroupedParams p) {
+                           const typename std::conditional<GRAD, ConvGroupedGradParams, ConvGroupedParams>::type p) {
   static_assert(MC == 1 || MC == 2 || MC == 4, "channels per thread");
   constexpr int KC = 512;   // gemm_simt_kernel.inc: 2048 / sizeof(float)
   constexpr int PX = CONV_GROUPED_PX;
@@ -607,25 +629,61 @@ conv_grouped_direct_kernel(float *__restrict__ out, const float *__restrict__ in
     const int x0 = xt * PX * p.XT, oh0 = yt * p.TY, m0 = mt * MB;
     const int ih0 = oh0 * p.sH - p.pH, iw0 = x0 * p.sW - p.pW;
     const float *src = in + (img * p.C + static_cast<int64_t>(g) * p.Cg) * HW;
-    const float *wsrc = wts + (static_cast<int64_t>(g) * p.Mg + m0) * p.Cg * taps;
+    const float *wsrc = GRAD ? wts + static_cast<int64_t>(g) * p.Cg * p.Mg * taps
+                             : wts + (static_cast<int64_t>(g) * p.Mg + m0) * p.Cg * taps;
     float acc[MC][PX], v[MC][PX];
 #pragma unroll
     for (int c = 0; c < MC; ++c)
 #pragma unroll
       for (int j = 0; j < PX; ++j) { acc[c][j] = 0.0f; v[c][j] = 0.0f; }
+    if constexpr (GRAD) {   // beta * dX as the exact kernel's first block takes it (beta = 0: dX is not read)
+      const int oh = oh0 + ty;
+      if (p.beta != 0.0f && oh < p.outH) {
+#pragma unroll
+        for (int c = 0; c < MC; ++c) {
+          const int m = m0 + cg * MC + c;
+          if (m >= p.Mg) continue;
+          const float *orow = out + ((img * p.G * p.Mg + static_cast<int64_t>(g) * p.Mg + m) * p.outH + oh) * p.outW;
+#pragma unroll
+          for (int j = 0; j < PX; ++j) {
+            const int ow = x0 + tx + j * p.XT;
+            if (ow < p.outW) v[c][j] = p.beta == 1.0f ? orow[ow] : __fmul_rn(orow[ow], p.beta);
+          }
+        }
+      }
+    }
     int kc = 0;   // k-steps of the current chain
     for (int ci = 0; ci < p.Cg; ++ci) {
       __syncthreads();   // the previous channel's patch and taps are consumed
       for (int i = tid; i < taps * MB; i += nthr) {
         const int tap = i / MB, mm = i - tap * MB;
-        ws[i] = m0 + mm < p.Mg ? wsrc[(static_cast<int64_t>(mm) * p.Cg + ci) * taps + tap] : 0.0f;
+        if constexpr (GRAD)   // W'_g: source channel ci's filter for output channel m0 + mm, rotated by 180 degrees
+          ws[i] = m0 + mm < p.Mg ? wsrc[(static_cast<int64_t>(ci) * p.Mg + m0 + mm) * taps + (taps - 1 - tap)] : 0.0f;
+        else
+          ws[i] = m0 + mm < p.Mg ? wsrc[(static_cast<int64_t>(mm) * p.Cg + ci) * taps + tap] : 0.0f;
       }
       const float *sc = src + ci * HW;
-      for (int i = tid; i < patch_words; i += nthr) {
-        const int pr = i / p.PC, pc = i - pr * p.PC;
-        const int ih = ih0 + pr, iw = iw0 + pc;
-        patch[i] = (static_cast<unsigned>(ih) < static_cast<unsigned>(p.H) && static_cast<unsigned>(iw) < static_cast<unsigned>(p.W))
-                       ? sc[static_cast<int64_t>(ih) * p.W + iw] : 0.0f;
+      if constexpr (GRAD) {
+        const float *ac = p.aux ? p.aux + (sc - in) : nullptr;
+        for (int i = tid; i < patch_words; i += nthr) {
+          const int pr = i / p.PC, pc = i - pr * p.PC;
+          const int h = ih0 + pr, w = iw0 + pc;   // in the dilated plane
+          const int hq = h / p.dH, wq = w / p.dW;
+          float x = 0.0f;
+          if (h >= 0 && w >= 0 && hq * p.dH == h && wq * p.dW == w && hq < p.H && wq < p.W) {
+            const int64_t off = static_cast<int64_t>(hq) * p.W + wq;
+            x = sc[off];
+            if (p.op != 0) x = operand_op(p.op, x, ac ? ac[off] : 0.0f);
+          }
+          patch[i] = x;
+        }
+      } else {
+        for (int i = tid; i < patch_words; i += nthr) {
+          const int pr = i / p.PC, pc = i - pr * p.PC;
+          const int ih = ih0 + pr, iw = iw0 + pc;
+          patch[i] = (static_cast<unsigned>(ih) < static_cast<unsigned>(p.H) && static_cast<unsigned>(iw) < static_cast<unsigned>(p.W))
+                         ? sc[static_cast<int64_t>(ih) * p.W + iw] : 0.0f;
+        }
       }
       __syncthreads();
       const float *prow = patch + ty * p.sH * p.PC + tx * p.sW;
@@ -635,7 +693,11 @@ conv_grouped_direct_kernel(float *__restrict__ out, const float *__restrict__ in
 #pragma unroll
             for (int c = 0; c < MC; ++c)
 #pragma unroll
-              for (int j = 0; j < PX; ++j) { v[c][j] = __fadd_rn(v[c][j], acc[c][j]); acc[c][j] = 0.0f; }
+              for (int j = 0; j < PX; ++j) {
+                if constexpr (GRAD) v[c][j] = __fadd_rn(v[c][j], p.alpha == 1.0f ? acc[c][j] : __fmul_rn(p.alpha, acc[c][j]));
+                else v[c][j] = __fadd_rn(v[c][j], acc[c][j]);
+                acc[c][j] = 0.0f;
+              }
             kc = 0;
           }
           ++kc;
@@ -673,9 +735,13 @@ conv_grouped_direct_kernel(float *__restrict__ out, const float *__restrict__ in
         for (int j = 0; j < PX; ++j) {
           const int ow = x0 + tx + j * p.XT;
           if (ow >= p.outW) continue;
-          float y = __fadd_rn(v[c][j], acc[c][j]);
-          if (p.bias != nullptr || p.act != 0) y = simt_bias_act(y, p.bias, 1, p.act, co, 0);
-          orow[ow] = y;
+          if constexpr (GRAD) {
+            orow[ow] = __fadd_rn(v[c][j], p.alpha == 1.0f ? acc[c][j] : __fmul_rn(p.alpha, acc[c][j]));
+          } else {
+            float y = __fadd_rn(v[c][j], acc[c][j]);
+            if (p.bias != nullptr || p.act != 0) y = simt_bias_act(y, p.bias, 1, p.act, co, 0);
+            orow[ow] = y;
+          }
         }
       }
     }

@@ -17,6 +17,7 @@
                                                   tap rows transposed out of the images in the operand preparation
     conv2d_input_grad_fused                       its input gradient, the transposed window gather over grad_output folded
                                                   into the operand preparation
+    conv2d_grouped_input_grad_fused               the input gradient of conv2d_grouped_fused: every group in one call
     conv2d_nhwc_input_grad_fused                  the input gradient of conv2d_nhwc_fused: NHWC gradients, the transposed
                                                   windows gathered along the channels in the operand preparation
     gemm_strided_batched                          (roadmap item of the reference, README.md:253-263)
@@ -37,6 +38,7 @@ FOREACH_OPS = {"copy": 0, "fill": 1, "scale": 2, "add": 3, "sub": 4, "mul": 5, "
 
 __all__ = ["forEach", "FOREACH_OPS", "transpose2D_copy", "transpose2D_batched", "nchw2nhwc", "nhwc2nchw", "conv2d_out_shape",
            "im2col_workspace_size", "im2col", "conv2d_im2col", "conv2d_fused", "conv2d_grouped_fused", "conv2d_filter_grad_fused", "conv2d_input_grad_fused",
+           "conv2d_grouped_input_grad_fused",
            "gemm_strided_batched", "copyFrom"]
 
 _i64 = ctypes.c_int64
@@ -268,6 +270,28 @@ def conv2d_input_grad_fused(grad_input, ishape, grad_output, kernel, kshape, pad
     check(lib().laser_b200_conv2d_input_grad_f32_fused_dev(pg, _i4(ishape), po, pk, _i4(kshape), _i2(padding), _i2(strides),
                                                            float(alpha), float(beta), ctypes.byref(o) if o is not None else None,
                                                            int(path), stream))
+
+
+def conv2d_grouped_input_grad_fused(grad_input, ishape, grad_output, kernel, kshape, padding, strides, groups, alpha=1.0, beta=0.0,
+                                    op=None, aux=None, path=PATH_AUTO, stream=None):
+    """conv2d_input_grad_fused with `groups` groups, as torch.nn.grad.conv2d_input(groups=groups), on float32 DEVICE buffers:
+    the input gradient of conv2d_grouped_fused (grad_input dense NCHW of shape ishape, grad_output dense NCHW, kernel
+    [c_out, c_in / groups, kH, kW]).  op and aux as for conv2d_input_grad_fused.  One call for every group: the direct
+    CUDA-core kernel over the transposed geometry on the exact path (depthwise and narrow groups), one batched tensor-core
+    GEMM launch per chunk on the others.  groups=1 is conv2d_input_grad_fused."""
+    pg, po, pk = _dev_f32(grad_input), _dev_f32(grad_output), _dev_f32(kernel)
+    o = None
+    if op is not None:
+        o = OperandOp()
+        o.op = OP_NAMES[op]
+        if aux is not None:
+            _, _, oh, ow = conv2d_out_shape(ishape, kshape, padding, strides)
+            o.aux = _dev_f32(aux)
+            o.auxRowStride, o.auxColStride = oh * ow, 1
+    stream = _current_stream() if stream is None else stream
+    check(lib().laser_b200_conv2d_grouped_input_grad_f32_fused_dev(pg, _i4(ishape), po, pk, _i4(kshape), _i2(padding), _i2(strides),
+                                                                   int(groups), float(alpha), float(beta),
+                                                                   ctypes.byref(o) if o is not None else None, int(path), stream))
 
 
 def conv2d_nhwc_input_grad_fused(grad_input, ishape, grad_output, kernel, kshape, padding, strides, alpha=1.0, beta=0.0, op=None,

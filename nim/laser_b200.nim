@@ -315,6 +315,12 @@ proc laser_b200_conv2d_input_grad_f32_fused_dev*(grad_input: ptr float32, ishape
                                                  grad_output, kernel: ptr float32, kshape: ptr array[4, int64],
                                                  padding, strides: ptr array[2, int64], alpha, beta: float32,
                                                  op: ptr LaserB200OperandOp, path: cint, stream: pointer): cint
+# the same with groups > 1 (torch.nn.grad.conv2d_input(groups=...)): kernel [c_out][c_in / groups][kH][kW]; groups = 1 is the
+# call above
+proc laser_b200_conv2d_grouped_input_grad_f32_fused_dev*(grad_input: ptr float32, ishape: ptr array[4, int64],
+                                                         grad_output, kernel: ptr float32, kshape: ptr array[4, int64],
+                                                         padding, strides: ptr array[2, int64], groups: int64, alpha, beta: float32,
+                                                         op: ptr LaserB200OperandOp, path: cint, stream: pointer): cint
 # the input gradient of the channels-last call: grad_input (NHWC) <- alpha * R * W'^T + beta * grad_input over every NHWC image
 # at once, A's windows over op(grad_output) prepared from the NHWC gradients; kernel as the forward call reads it
 proc laser_b200_conv2d_nhwc_input_grad_f32_fused_dev*(grad_input: ptr float32, ishape: ptr array[4, int64],
